@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — decoded frames/s of openHEVC's pixel-reconstruction path on B200 (driver contract).
+"""bench.py — decoded frames/s of openHEVC's pixel-reconstruction path on H100 GPUs.
 
 Workload (BASELINE.json configs[2]/[3]): 3840x2160 Main10 4:2:0 random-access stream, hierarchical-B GOP 8,
 intra period 32, synthetic work lists (openhevc_b200/synth.py, SURVEY.md §8d).  One *step* = one GOP
 (8 pictures) per rank; pictures of GOP g are decoded by rank g mod N, anchors are broadcast over NCCL
 (openhevc_b200/frame_parallel.py).  `value` = pictures/s with all work lists resident in HBM;
 `e2e` = the same through the host-facing C ABI: pinned host blob -> H2D -> K1..K5 -> D2H of the picture.
+--dump-outputs DIR writes the pictures of the last timed GOP of rank 0 as DIR/<name>.npy (float32).
 """
 import argparse
 import json
@@ -282,6 +283,8 @@ def run_reference(args, wl, rank):
     same work lists on the host cores, frame-parallel over pthreads like its frame threads."""
     if rank != 0:
         return
+    if args.dump_outputs:
+        print("bench.py: --dump-outputs applies to the GPU path only; the reference arm writes nothing", file=sys.stderr)
     import oracle_lib
     from openhevc_b200.synth import smooth_frame
     if oracle_lib.ref_lib() is None:
@@ -329,6 +332,36 @@ def run_reference(args, wl, rank):
     print(json.dumps(line), file=_REAL_STDOUT, flush=True)
 
 
+DUMP_SAMPLES = 1 << 19        # per plane: 8 pictures x 3 planes x 2 MB of float32 stay under 64 MB
+
+
+def dump_outputs(out_dir, eng, FP, rank, world, steps):
+    """the pictures of the last GOP of the timed schedule on this rank, read back from their DPB slots (nothing later writes
+    them); a plane larger than DUMP_SAMPLES is stored flat as a fixed, seeded sample of DUMP_SAMPLES samples"""
+    class Record:
+        def __init__(self):
+            self.pics = []
+
+        def decode(self, pic, g=None):
+            self.pics.append((g, pic))
+
+        def exchange_anchors(self, *a):
+            pass
+    rec = Record()
+    FP.run_schedule(rec, rank, world, steps)
+    g_last = max(g for g, _ in rec.pics)
+    os.makedirs(out_dir, exist_ok=True)
+    eng.sync()
+    for k, pic in enumerate(p for g, p in rec.pics if g == g_last):
+        planes = eng.readback(pic.cur_slot)
+        for p, (name, a) in enumerate(zip(("y", "cb", "cr"), planes)):
+            a = a.astype(np.float32)
+            if a.size > DUMP_SAMPLES:
+                idx = np.sort(np.random.default_rng(3 * k + p).choice(a.size, DUMP_SAMPLES, replace=False))
+                a = a.reshape(-1)[idx]
+            np.save(os.path.join(out_dir, f"gop{g_last}_pic{k}_{name}.npy"), a)
+
+
 _REAL_STDOUT = sys.stdout
 
 
@@ -341,13 +374,14 @@ def main():
     os.dup2(2, 1)
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=512, help="GOPs (8 pictures) per rank in the timed region (512: > 1 s at 4K)")
+    ap.add_argument("--steps", type=int, default=512, help="GOPs (8 pictures) per rank in the timed region (several ranks: rounded up to 4)")
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="c3_4k_main10_ra", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-stream", action="store_true", help="skip the real-decoder stream block (e2e falls back to the work-list replay)")
     ap.add_argument("--streams", default="headline,mid,dense,modes", help="which streams the stream_e2e block decodes")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the pictures of the last timed GOP (rank 0) to DIR/<name>.npy")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -411,7 +445,9 @@ def main():
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms = float(ms.item())
-    n_total = n_mine * world                     # (whole intra periods per rank: steps is rounded up to a multiple of 4 GOPs)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, FP, rank, world, args.steps)
+    n_total = n_mine * world
     fps = n_total / (ms * 1e-3)
 
     # ---- per-stage times of every distinct picture (CUDA events inside the library, on its compute stream) ----
@@ -436,24 +472,13 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3, 700 W card), not measured"
     stages = {k: {"ms": stage_ms[k], "algorithmic_bytes": abytes[k], "gbps": abytes[k] / (stage_ms[k] * 1e-3) / 1e9 if stage_ms[k] > 0 else None}
               for k in abytes}
     dom = max(abytes, key=lambda k: stage_ms[k])
-    # DRAM traffic of the dominant kernel from the committed ncu capture (profiles/ncu_traffic.json: one B picture, per launch)
-    traffic, traffic_note = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        kname = {"mc": "k_mc_v1<unsigned short, 32>", "residual": "k_residual<unsigned short>", "intra": "k_intra<unsigned short>",
-                 "deblock": "k_deblock<unsigned short>", "sao": "k_sao<unsigned short>"}[dom]
-        if wl["bit_depth"] > 8 and wl["width"] == 3840 and kname in tj["kernels"]:
-            traffic = tj["kernels"][kname]["dram_bytes_per_launch"]
-            traffic_note = "dram read+write bytes per launch of " + kname + " on a 4K B picture, " + tj["source"]
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": {"mc": "k_mc", "residual": "k_residual", "intra": "k_intra", "deblock": "k_deblock", "sao": "k_sao"}[dom],
                 "achieved": stages[dom]["gbps"], "peak": peak, "unit": "GB/s", "frac": stages[dom]["gbps"] / peak, "peak_source": peak_src,
-                "traffic": traffic, "traffic_note": traffic_note, "share_of_step": stage_ms[dom] / stage_ms["total"], "stages": stages,
+                "share_of_step": stage_ms[dom] / stage_ms["total"], "stages": stages,
                 "stage_ms_by_picture": stage_by_blob, "intra_levels": {FP.blob_specs()[b][0] + f"#{b}": (stats[b].get("intra_levels"), stats[b].get("intra_levels_in_ctb")) for b in range(FP.N_BLOBS)},
                 "whole_picture": {"algorithmic_bytes": sum(abytes.values()), "ms": stage_ms["total"],
                                   "gbps": sum(abytes.values()) / (stage_ms["total"] * 1e-3) / 1e9}}
@@ -550,7 +575,7 @@ def main():
                         "md5_equal_reference_decoder": mine["b200"].get("md5_equal_reference_decoder")}
 
     if rank == 0:
-        line = {"metric": METRIC, "value": fps, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
+        line = {"metric": METRIC, "value": fps, "unit": UNIT, "n_gpus": world, "steps": n_mine // 8, "warmup": args.warmup,
                 "ms_per_step": ms / (n_mine / 8), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "u16" if wl["bit_depth"] > 8 else "u8", "data": "synthetic",
                 "config": workload_config(args.workload, wl, world),

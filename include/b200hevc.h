@@ -1,5 +1,5 @@
 /*
- * b200hevc.h — C ABI of libb200hevc.so, the B200 (sm_100a) back end for openHEVC's
+ * b200hevc.h — C ABI of libb200hevc.so, the H100 (sm_90a) back end for openHEVC's
  * per-CTU pixel-reconstruction path.
  *
  * Layering (see DESIGN.md):

@@ -1,4 +1,4 @@
-"""openhevc_b200 — B200 (sm_100a) back end for openHEVC's per-CTU pixel-reconstruction path.
+"""openhevc_b200 — H100 (sm_90a) back end for openHEVC's per-CTU pixel-reconstruction path.
 
 The product is the C-ABI library `libb200hevc.so` (include/b200hevc.h) plus the table shim that
 re-populates the reference's HEVCDSPContext / HEVCPredContext (include/b200hevc_tables.h).  This

@@ -24,7 +24,7 @@ HD int clip16i(int v) { return v < -32768 ? -32768 : v > 32767 ? 32767 : v; }
 HD int imin(int a, int b) { return a < b ? a : b; }
 HD int imax(int a, int b) { return a > b ? a : b; }
 
-// ---- 16x2 SIMD integer helpers: the sm_100a instructions (VIADD.16x2, VIADDMNMX.S16x2.RELU, VIMNMX.U16x2, PRMT, SHF)
+// ---- 16x2 SIMD integer helpers: the sm_90a (DPX) instructions (VIADD.16x2, VIADDMNMX.S16x2.RELU, VIMNMX.U16x2, PRMT, SHF)
 // on the device, their definition in plain C on the host ----
 HD uint32_t prmt32(uint32_t a, uint32_t b, uint32_t sel)          // prmt.b32, generic mode, selectors 0..7 only
 {

@@ -289,7 +289,7 @@ static int ctx_init(B200Ctx *ctx)
     CU(cudaSetDevice(c.device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, c.device));
-    if (prop.major < 10) return fail(ctx, B200_ENOTSUP, "device %d is sm_%d%d; this library carries sm_100a code only", c.device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(ctx, B200_ENOTSUP, "device %d is sm_%d%d; this library carries sm_90a code only", c.device, prop.major, prop.minor);
     geometry(&c, ctx->pw, ctx->ph, ctx->pitch, ctx->plane_off, &ctx->slot_bytes);
     const uint64_t need = (uint64_t)ctx->slot_bytes * c.n_slots;
     if (c.ext_frame_mem) {
@@ -467,7 +467,7 @@ static int validate_mode()
     return mode;
 }
 
-// host-side validation (every record in range), ~1 ms of host time for a 4K picture: B200_VALIDATE=2.  The default is the
+// host-side validation (every record in range), on the submitting thread: B200_VALIDATE=2.  The default is the
 // same set of checks on the device (k_validate in kernels.cu) -- keep the two in step.
 static int deep_check(B200Ctx *ctx, const uint8_t *blob)
 {
@@ -569,7 +569,7 @@ extern "C" int b200_frame_upload(B200Ctx *ctx, const void *blob, uint64_t nbytes
     if (rc) { ctx->err_code = 0; return rc; }
     // every record is validated before it is used: by default on the device, in front of the picture's kernels
     // (k_validate, a few microseconds; errors surface from b200_sync like the other device-side errors);
-    // B200_VALIDATE=2 checks on the host instead (synchronous error from this call, ~1 ms per 4K picture), 0 = off
+    // B200_VALIDATE=2 checks on the host instead (synchronous error from this call), 0 = off
     if (validate_mode() == 2 && (rc = deep_check(ctx, (const uint8_t *)blob))) { ctx->err_code = 0; return rc; }
     CU(cudaSetDevice(ctx->cfg.device));
     Arena &a = ctx->arena[arena];

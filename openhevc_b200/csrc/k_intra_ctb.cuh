@@ -1,6 +1,6 @@
 // k_intra_ctb.cuh — K3, CTB-granular: one thread block per CTB, the CTB's samples in shared memory.
 //
-// The TU-granular stage (k_intra, kernels.cu) pays one L2 round trip per dependent transform block: ~1 us per step of a
+// The TU-granular stage (k_intra, kernels.cu) pays one L2 round trip per dependent transform block, on each step of a
 // ~3400-step chain on a 4K intra picture.  Most of those steps stay inside one CTB.  Here a block owns a CTB:
 //   * the CTB's reconstruction (all three planes), its residuals and its records are staged in shared memory while the block
 //     waits for its neighbour CTBs -- left, up-left, up, up-right: the wavefront of hevc.c:2751-2832 -- whose borders it then

@@ -11,8 +11,8 @@
 //   B  vertical FIR (if my) or pass-through: lane = column, up to 8 rows per lane -> val[0..7] in registers.
 // then the uni / bi / weighted combine and the store.
 //
-// The stage is issue-bound (profiles/): the FIRs are therefore written for IDP.2A, the two-way 16-bit x 8-bit dot
-// product of sm_100a -- two taps per instruction on samples that stay packed in pairs:
+// The stage is issue-bound: the FIRs are therefore written for IDP.2A, the two-way 16-bit x 8-bit dot
+// product of sm_90a -- two taps per instruction on samples that stay packed in pairs:
 //   * stage A reads six aligned 32-bit words (12 samples) per lane and row; outputs whose first tap falls on an even
 //     sample use the words as they are, the others use the five pairs shifted by one sample (PRMT); an 8-tap output
 //     is 4 IDP.2A (lo / hi halves of two coefficient registers) instead of 8 IMAD;

@@ -5,8 +5,7 @@
 #include "common.cuh"
 
 #ifndef SAO_R
-#define SAO_R 2          // rows per thread.  Round 2, measured (gpurun_out/b9_sao.txt): 2 rows + 3 blocks per SM beats 4 rows + 2 blocks
-                         // by 4-6 % on the filter-only sweep (8K 4:2:2: 0.413 -> 0.427 of HBM peak, 4K: 0.375 -> 0.399): more warps to hide the loads
+#define SAO_R 2          // rows per thread: 2 rows + 3 blocks per SM leave more warps to hide the loads than 4 rows + 2 blocks
 #endif
 
 // 8 consecutive samples (x multiple of 8: 16-byte / 8-byte aligned; rows are padded to the pitch, so a vector that

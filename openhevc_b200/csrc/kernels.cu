@@ -1,4 +1,4 @@
-// kernels.cu — hand-written sm_100a kernels for openHEVC's pixel-reconstruction path.
+// kernels.cu — hand-written sm_90a kernels for openHEVC's pixel-reconstruction path.
 //
 // One kernel per stage, each consuming one section of the per-frame work list
 // (include/b200hevc_worklist.h):
@@ -324,7 +324,7 @@ __device__ __forceinline__ void residual_warp(const B200TuRec *__restrict__ recs
 }
 
 // All four TU sizes in ONE launch: separate launches ran back to back although none of them fills the machine (the
-// 32x32 list is a few hundred CTAs at 14 % occupancy for 23 us).  Largest TUs first, so that the long-running warps
+// 32x32 list is a few hundred CTAs).  Largest TUs first, so that the long-running warps
 // start first and the small ones fill in behind them.
 struct ResidualLists {
     const B200TuRec *recs[4];            // 4x4, 8x8, 16x16, 32x32
@@ -1069,7 +1069,7 @@ __global__ void k_intra_edges_init(FrameDesc f, IntraEdges ed)
 
 // The same, driven by the intra records: only the units an intra TU can read (the row above from the up-left corner to the
 // end of the up-right block, the column to the left down to the end of the bottom-left block) are initialised -- a B
-// picture with 8 % intra blocks touches a few per cent of the picture instead of reading all of it (25 MB, 11 us at 4K).
+// picture with 8 % intra blocks touches a few per cent of the picture instead of reading all of it (25 MB at 4K).
 // One warp per record, lane k = unit k of the 4u + 1 neighbours.  Units that belong to another intra TU get a record from
 // the picture as well; k_intra_prepass, which runs after this kernel, marks them "not valid yet" again.
 template <typename PIX>
@@ -1109,7 +1109,7 @@ __global__ void k_intra_prepass(const B200IntraRec *__restrict__ recs, int count
 
 // Poll until every lane of the warp has its record(s).  Executed by all 32 lanes with a uniform (vote) exit so the
 // warp leaves the loop CONVERGED -- a per-lane `while (!valid)` lets lanes leave one by one and the rest of the TU
-// then runs as diverged fragments (measured 5100 vs ~700 cycles for a 4x4 TU).  A malformed list (dependency cycle)
+// then runs as diverged fragments, several times slower.  A malformed list (dependency cycle)
 // must not hang the GPU: give up after ~0.3 s and latch an error in counter[2].
 // `pa_alt`: alternative source of record a (the up-left corner sample is the last element of BOTH halves of its unit,
 // and depending on the neighbour's geometry only the bottom row or only the right column of that unit is published).
@@ -1491,7 +1491,7 @@ __global__ void __launch_bounds__(DBK_THREADS, 3) k_deblock(const uint16_t *__re
 //
 // The stage is issue-bound, not bandwidth-bound, so the kernel is written around the instruction count:
 //  * samples stay packed two per 32-bit register (16-bit halves; 8-bit pictures are widened on load) and are
-//    classified with the 16x2 SIMD integer instructions of sm_100a (VIADD.16x2, VIADDMNMX.S16x2.RELU):
+//    classified with the 16x2 SIMD integer (DPX) instructions of sm_90a (VIADD.16x2, VIADDMNMX.S16x2.RELU):
 //    sign(c - a) + 1 = relu(min(c + (1 - a), 2)) is ONE instruction for two samples;
 //  * the offset is fetched with a byte permute (PRMT) from a 5-entry table held in two registers (offsets biased by
 //    128: |offset| <= 124 for every legal stream up to 12 bits, hevc_cabac.c:684-692 / hevc.c:1178);
@@ -1531,7 +1531,14 @@ __global__ void k_fill(FrameDesc f, int value)
 // --------------------------------------------------------------------------------------------
 // launchers
 // --------------------------------------------------------------------------------------------
-static void mc4_opt_in()                 // more than 48 KB of dynamic shared memory per block: once per kernel
+static int sm_count()                    // SMs of the current device: the persistent grids below are sized per SM
+{
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n > 0 ? n : 1;
+}
+static void mc4_opt_in()               // more than 48 KB of dynamic shared memory per block: once per kernel
 {
     static bool done = false;
     if (done) return;
@@ -1544,7 +1551,7 @@ static void mc4_opt_in()                 // more than 48 KB of dynamic shared me
 static int mc4_grid(int blocks_needed)   // persistent blocks: a few per SM (B200_MC4_CTAS per SM, default 3), never more than the work
 {
     static const int per_sm = getenv("B200_MC4_CTAS") ? atoi(getenv("B200_MC4_CTAS")) : 3;
-    const int cap = 148 * (per_sm > 0 ? per_sm : 3);
+    const int cap = sm_count() * (per_sm > 0 ? per_sm : 3);
     return blocks_needed < cap ? blocks_needed : cap;
 }
 
@@ -1552,18 +1559,14 @@ int launch_mc(cudaStream_t st, const B200McRec *recs, int count, int n_big, cons
               const FrameDesc &slot0, unsigned long long slot_bytes)
 {
     if (!count) return 0;
-    // B200_MC_DESC=1: reference planes described from kernel parameters (see DpbLayout); default 0 = descriptor table, the
-    // path every GPU run of round 1 used -- the switch exists so that the next GPU visit can measure the difference at once
+    // B200_MC_DESC=1: reference planes described from kernel parameters (see DpbLayout); default 0 = descriptor table
     static const bool by_param = getenv("B200_MC_DESC") && atoi(getenv("B200_MC_DESC"));
     static const int tmp_pad = getenv("B200_MC_PAD") ? atoi(getenv("B200_MC_PAD")) : 0;
     DpbLayout lay;
     lay.slot0 = slot0; lay.slot_bytes = by_param ? slot_bytes : 0ull; lay.tmp_pad = tmp_pad;
-    // 1 = scalar FIRs, one IMAD per tap (default); 2 = IDP.2A on packed pairs (k_mc.cuh).  Version 2 is bit-exact on the GPU
-    // (full parity suite) but SLOWER: 145 vs 109 us per 4K B picture, 38.9 M + 29.7 M vs 35.4 M + 22.8 M warp instructions --
-    // the pair shuffles and the 16-bit interleaved stores cost more than the halved multiplies save, and ncu shows the
-    // stage waiting on its window loads (long scoreboard), not on the ALU.  Kept selectable for the next round's work.
-    // 3 = version 1's arithmetic with the window loads of both lists issued back to back (k_mc_v3): written after the last GPU
-    // visit of round 1, bit-exact in the warp emulation (tests/test_warp_emul_cpu.py), 80 registers / 3 CTAs per SM; not yet timed.
+    // 1 = scalar FIRs, one IMAD per tap (default); 2 = IDP.2A on packed pairs (k_mc.cuh), bit-exact; its pair shuffles and
+    // 16-bit interleaved stores add instructions the halved multiplies have to pay back.
+    // 3 = version 1's arithmetic with the window loads of both lists issued back to back (k_mc_v3).
     // 4 = persistent groups, windows double-buffered through 16-byte cp.async, descriptors from kernel parameters (k_mc_v4)
     static const int version = getenv("B200_MC") ? atoi(getenv("B200_MC")) : 1;
     DpbLayout lay4;
@@ -1648,7 +1651,7 @@ int launch_intra(cudaStream_t st, const B200IntraRec *recs, int count, const int
     for (int p = 0; p < 3; p++) { ed.e[p] = edges[p]; ed.stride[p] = edge_stride[p]; }
     // counter[0] (ticket) and counter[1] (gate) were cleared when the picture entered its lane (engine.cu)
     // B200_EDGES_SPARSE=1: initialise only the edge records intra TUs can read (record-driven) when the picture is mostly inter;
-    // default 0 = every unit of the picture, the path every GPU run of round 1 used (switch for the next GPU visit)
+    // default 0 = every unit of the picture
     static const bool sparse_ok = getenv("B200_EDGES_SPARSE") && atoi(getenv("B200_EDGES_SPARSE"));
     const long units = (long)(cur.p[0].w / 4) * (cur.p[0].h / 4) + 2l * (cur.p[1].w / 4) * (cur.p[1].h / 4);
     if (sparse_ok && (long)count * 16 < units) {
@@ -1663,10 +1666,9 @@ int launch_intra(cudaStream_t st, const B200IntraRec *recs, int count, const int
     int grid = (count + 3) / 4;
     // persistent warps.  The list is sorted by dependency level, so the TUs that can run together are adjacent and a
     // small window exposes all the parallelism there is; more waiting warps only take issue slots from the other pictures
-    // in flight.  Measured on a B200 (4K Main10 RA mix, 8 lanes; gpurun_out/b10_*, b12_*), pictures/s with 1184 / 592 / 296 /
-    // 148 / 74 blocks: 2980 / 3507 / 3842 / 4027 / 4045; the I picture takes 4.07 ms down to 148 blocks and 4.19 ms with 74,
-    // the intra blocks of a B picture 70 / 75 / 90 / 116 / 174 us when timed alone.  One block per SM.
-    static const int max_ctas = getenv("B200_INTRA_CTAS") ? atoi(getenv("B200_INTRA_CTAS")) : 148;
+    // in flight, while far fewer blocks than SMs lengthen the serial chain of an I picture.  One block per SM.
+    static const int env_ctas = getenv("B200_INTRA_CTAS") ? atoi(getenv("B200_INTRA_CTAS")) : 0;
+    const int max_ctas = env_ctas > 0 ? env_ctas : sm_count();
     if (grid > max_ctas) grid = max_ctas;
     CipDesc cd;
     memset(&cd, 0, sizeof(cd));
@@ -1700,7 +1702,8 @@ int launch_intra_ctb(cudaStream_t st, const B200IntraRec *recs, int count, const
         a.rt_stride[p] = cw;
         a.rt_off[p] = off; off += (cw * ch * 2 + 15) & ~15;
     }
-    int grid = a.n_ctb < 148 * 2 ? a.n_ctb : 148 * 2;
+    const int cap = 2 * sm_count();
+    int grid = a.n_ctb < cap ? a.n_ctb : cap;
     static const int max_ctas = getenv("B200_INTRA_CTAS") ? atoi(getenv("B200_INTRA_CTAS")) : 0;
     if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
     static bool attr_set[2] = { false, false };

@@ -760,10 +760,8 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
         static thread_local std::vector<uint32_t> perm;
         static thread_local std::vector<uint8_t> lev;
         // 1 (default): picture-wide level order, TU-granular wavefront (k_intra); 2: CTB order, CTB-granular stage (k_intra_ctb.cuh).
-        // Measured on a B200 (round 2, 4K Main10): the CTB-granular stage is bit-exact (whole GPU suite) but SLOWER -- 11.6 ms for an
-        // intra picture against 4.07 ms, 1.2 ms against 0.09 ms for the intra blocks of a B picture: a CTB has up to ~80 dependency
-        // levels and a level costs ~1 us either way (the dependent instruction chain of one block, not the memory hop), so waiting
-        // for whole neighbour CTBs triples the number of serial steps (~10 k against the ~3.4 k of the block-level graph).
+        // The CTB-granular stage is bit-exact but has more serial steps: a CTB has up to ~80 dependency levels, and waiting for whole
+        // neighbour CTBs turns the ~3.4 k steps of the block-level graph of a 4K intra picture into ~10 k.
         static const int intra_mode = getenv("B200_INTRA") ? atoi(getenv("B200_INTRA")) : 1;
         perm.resize(r->intra.size());
         B200IntraRec *dst = (B200IntraRec *)(r->blob + o);

@@ -69,21 +69,20 @@ def period_owner(q, world):
     return q % world
 
 
-def period_pictures(q, k=None):
+def period_pictures(q, k=None, n_gops=INTRA_PERIOD_GOPS):
     """The pictures of intra period q in the order its owner issues them, and which of them waits for the one picture that
-    comes from another GPU.
+    comes from another GPU.  n_gops < INTRA_PERIOD_GOPS: only the first n_gops GOPs of the period (the end of a run).
 
-    A period starts with an I anchor, so its anchor chain I -> P -> P -> P never leaves the GPU (round 1 gave GOP g to rank
-    g mod N: every anchor then waited for the previous GOP's anchor on another GPU, decode -> broadcast -> decode in series:
-    efficiency 0.41 at 8 GPUs).  The stream is open-GOP: the seven B pictures in front of the I anchor (output order) still
-    reference the LAST anchor of the previous period.  They are leaves -- nothing references them -- so the owner issues them
+    A period starts with an I anchor, so its anchor chain I -> P -> P -> P never leaves the GPU (giving GOP g to rank g mod N
+    would make every anchor wait for the previous GOP's anchor on another GPU: decode -> send -> decode in series).  The stream
+    is open-GOP: the seven B pictures in front of the I anchor (output order) still reference the LAST anchor of the previous period.  They are leaves -- nothing references them -- so the owner issues them
     last, when that anchor has long arrived (it is the 4th of the 4 anchors of the neighbour's period, which runs at the same
     time).  k: index of the period among the periods of its GPU (slot rotation; default q).
     Returns [(global GOP index, Picture, needs_prev_period_anchor)]."""
     k = q if k is None else k
     g0 = q * INTRA_PERIOD_GOPS
     out, deferred = [], []
-    for g in range(g0, g0 + INTRA_PERIOD_GOPS):
+    for g in range(g0, g0 + n_gops):
         pics = gop_pictures(g, k * INTRA_PERIOD_GOPS + (g - g0), 2 if g == g0 else (g - g0) & 1)
         out.append((g, pics[0], False))
         if g == g0:
@@ -95,18 +94,20 @@ def period_pictures(q, k=None):
 
 def run_schedule(backend, rank, world, n_gops_per_rank):
     """Issue the whole schedule (asynchronously on a GPU backend).  Returns pictures decoded by this rank.
-    n_gops_per_rank GOPs per rank = n_gops_per_rank / 4 intra periods per rank (a remainder is rounded up to whole periods:
-    the unit of ownership); period q goes to rank q mod N.  The one exchange per period: its owner receives the previous
+    n_gops_per_rank GOPs per rank = n_gops_per_rank / 4 intra periods per rank; period q goes to rank q mod N.  A remainder
+    cuts the last period short on one rank; with several ranks it is rounded up to a whole period, so that the GOPs decoded
+    are always the first ones of the stream.  The one exchange per period: its owner receives the previous
     period's last anchor from rank - 1 and sends its own last anchor to rank + 1 (point to point: exactly one GPU ever reads it)."""
     rounds = -(-n_gops_per_rank // INTRA_PERIOD_GOPS)
     n_periods = rounds * world
     decoded = 0
     for k in range(rounds):
         q = k * world + rank
+        n_gops = min(INTRA_PERIOD_GOPS, n_gops_per_rank - k * INTRA_PERIOD_GOPS) if world == 1 else INTRA_PERIOD_GOPS
         recv_slot = anchor_slot(k * INTRA_PERIOD_GOPS - 1) if (world > 1 and q > 0) else None
-        send_slot = anchor_slot(k * INTRA_PERIOD_GOPS + INTRA_PERIOD_GOPS - 1) if (world > 1 and q + 1 < n_periods) else None
+        send_slot = anchor_slot(k * INTRA_PERIOD_GOPS + n_gops - 1) if (world > 1 and q + 1 < n_periods) else None
         exchanged = False
-        for (g, pic, needs_prev) in period_pictures(q, k):
+        for (g, pic, needs_prev) in period_pictures(q, k, n_gops):
             if needs_prev and not exchanged:
                 # the last anchor of this period is decoded (the deferred pictures come after everything else): one grouped
                 # exchange, ordered on the device by the slots' hazards

@@ -47,8 +47,7 @@ sed -i -e '/^void ff_hevc_deblocking_boundary_strengths(HEVCContext \*s, int x0,
 # until the rows of a reference picture its motion vector reaches have been reconstructed by another thread -- for pixels nobody reads on
 # the host once the MC tables record (the device runs the pictures in decode order; the TMVP wait, hevc_mvs.c:260, would stay).  Bit-exact
 # (CPU suite, emulated device with 4 / 8 frame threads, MD5 on the GPU at 32 threads); host-only (record and drop, 8 cores) +5 % at 8 and
-# +12 % at 16 threads, but on the B200 box 886 vs 986 fps at 32 threads and 802 vs 808 at 16 (gpurun_out/b13_await_guard.txt): no gain
-# where it counts, so the decoder keeps its own synchronisation.
+# +12 % at 16 threads, but with the device no gain was measured, so the decoder keeps its own synchronisation.
 if [ -n "${B200_AWAIT_GUARD:-}" ]; then
   sed -i -e '/^static void hevc_await_progress(HEVCContext \*s, HEVCFrame \*ref,/,/^}/ s/^    int y = (mv->y >> 2) + y0 + height + 9;/&\n    if (b200_host_pixels_unused()) return;   \/* reference PIXELS are not read on the host *\//' "$P/hevc.c"
   grep -q "b200_host_pixels_unused()) return;   /\* reference PIXELS" "$P/hevc.c" || { echo "await guard was not inserted" >&2; exit 1; }
@@ -67,6 +66,6 @@ for f in hevc hevcdsp hevcpred videodsp hevc_refs hevc_filter utils; do
       -c "$P/$f.c" -o "$OUT/obj_b200/libavcodec_$f.o"
 done
 objs=$(ls "$OUT"/obj/*.o | grep -v -e 'libavcodec_hevc\.o' -e 'libavcodec_hevcdsp\.o' -e 'libavcodec_hevcpred\.o' -e 'libavcodec_videodsp\.o' -e 'libavcodec_hevc_refs\.o' -e 'libavcodec_hevc_filter\.o' -e 'libavcodec_utils\.o')
-gcc -shared -o "$OUT/libohevc_b200.so" $objs "$OUT"/obj_b200/*.o -L"$ROOT/openhevc_b200" -lb200hevc_shim -lb200hevc \
-    -Wl,-rpath,'$ORIGIN/../../openhevc_b200' -lm -lpthread
+gcc -shared -o "$OUT/libohevc_b200.so" $objs "$OUT"/obj_b200/*.o -L"$OUT" -lb200hevc_shim -L"$ROOT/openhevc_b200" -lb200hevc \
+    -Wl,-rpath,'$ORIGIN:$ORIGIN/../../openhevc_b200' -lm -lpthread
 echo "built $OUT/libohevc_b200.so"

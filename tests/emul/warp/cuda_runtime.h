@@ -4,7 +4,7 @@
 // fiber until every participating lane has arrived, exactly the contract the device gives; everything the runtime API does
 // asynchronously on a device (copies, memsets, kernels, events) happens immediately here.  The result is
 // oracle/_ref/libb200hevc_emul.so with the same C ABI as libb200hevc.so, loaded ONLY by tests/ (never by the product): the
-// CPU suite can run whole work lists and whole streams through the very kernel source that is compiled for sm_100a.
+// CPU suite can run whole work lists and whole streams through the very kernel source that is compiled for sm_90a.
 // What it cannot show: memory-model races, stream / event ordering, performance.
 #pragma once
 #ifndef B200_EMUL
@@ -182,5 +182,7 @@ static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSucces
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline const char *cudaGetErrorString(cudaError_t) { return "emulated CUDA runtime: no error"; }
-static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { memset(p, 0, sizeof(*p)); strcpy(p->name, "warp-lockstep CPU emulation"); p->multiProcessorCount = 1; p->major = 10; return cudaSuccess; }
+static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { memset(p, 0, sizeof(*p)); strcpy(p->name, "warp-lockstep CPU emulation"); p->multiProcessorCount = 132; p->major = 9; return cudaSuccess; }
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
+static inline cudaError_t cudaDeviceGetAttribute(int *v, cudaDeviceAttr a, int) { *v = a == cudaDevAttrMultiProcessorCount ? 132 : 0; return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetPCIBusId(char *s, int n, int) { if (n > 0) s[0] = 0; return cudaErrorInvalidValue; }

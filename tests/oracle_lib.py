@@ -1,6 +1,10 @@
 """TEST INFRASTRUCTURE: ctypes access to the CPU oracle (oracle/hevc_oracle.c) and helpers that
 compare the CUDA path with it.  Never imported by the product package."""
 import ctypes as C
+import glob
+import hashlib
+import io
+import lzma
 import os
 import subprocess
 
@@ -86,7 +90,7 @@ def ref_execute(blob, dpb):
     return planes[int(blob[23])]
 
 
-SHIM_SO = os.path.join(ROOT, "openhevc_b200", "libb200hevc_shim.so")
+SHIM_SO = os.path.join(ORACLE_DIR, "_ref", "libb200hevc_shim.so")
 
 
 def ref_execute_b200(blob, dpb):
@@ -151,3 +155,64 @@ def check_decode_order(blob):
             assert px >= 0 and py >= 0, f"intra TU {i} reads outside the picture"
             assert o[py // 4, px // 4] < i, f"intra TU {i} depends on later TU {o[py // 4, px // 4]}"
     return True
+
+
+WORKLIST_DIR = os.path.join(ROOT, "tests", "golden", "worklists")
+
+
+def md5_line(k, hdr, planes):
+    w, h, bd = int(hdr["width"]), int(hdr["height"]), int(hdr["bit_depth"])
+    md5 = [hashlib.md5((np.asarray(p).astype(np.uint8) if bd == 8 else np.asarray(p).astype("<u2")).tobytes()).hexdigest() for p in planes]
+    return f"frame {k} {w}x{h} bd{bd} " + " ".join(md5)
+
+
+def recorded_worklists(stream, threads="1"):
+    """work lists the hooked decoder recorded for a committed stream with `threads` ("1", "4", "4w"; golden/make_golden.py), or None"""
+    import zipfile
+    member = os.path.basename(stream).replace(".hevc", "") + {"1": "", "4": ".f4", "4w": ".w4"}[threads] + ".npz.xz"
+    for pack in sorted(glob.glob(os.path.join(WORKLIST_DIR, "pack_*.zip"))):
+        with zipfile.ZipFile(pack) as zf:
+            if member in zf.namelist():
+                z = np.load(io.BytesIO(lzma.decompress(zf.read(member))))
+                break
+    else:
+        return None
+    return dict(blobs=[z["blob"][a:b] for a, b in zip(z["off"][:-1], z["off"][1:])], out_idx=[int(v) for v in z["out_idx"]],
+                fills=[tuple(int(v) for v in f) for f in z["fills"]])
+
+
+def replay_worklists(rec, gpu):
+    """recorded work lists in decode order on one DPB, by the CUDA path or the CPU oracle: {output index: md5_line}"""
+    from openhevc_b200 import worklist as W
+    hdr, _ = W.parse_blob(rec["blobs"][0])
+    w, h, cfi, bd = int(hdr["width"]), int(hdr["height"]), int(hdr["chroma_format_idc"]), int(hdr["bit_depth"])
+    n_slots, lines = 32, {}
+    if gpu:
+        from openhevc_b200 import FrameEngine
+        eng = FrameEngine(w, h, cfi, bd, log2_ctb_size=int(hdr["log2_ctb_size"]), n_slots=n_slots)
+    else:
+        dpb = [[np.zeros(W.plane_dims(w, h, cfi, p)[::-1], np.uint16) for p in range(3)] for _ in range(n_slots)]
+    try:
+        for k, blob in enumerate(rec["blobs"]):
+            hdr, _ = W.parse_blob(blob)
+            for (pic, slot, value) in rec["fills"]:
+                if pic == k and gpu:
+                    eng.fill_slot(slot, value)
+                elif pic == k:
+                    dpb[slot] = [np.full_like(p, value) for p in dpb[slot]]
+            if gpu:
+                out = eng.decode(blob)
+            else:
+                out = execute(blob, dpb)
+                dpb[int(hdr["cur_slot"])] = out
+            lines[rec["out_idx"][k]] = md5_line(rec["out_idx"][k], hdr, out)
+    finally:
+        if gpu:
+            eng.close()
+    return lines
+
+
+def recorded_streams():
+    import zipfile
+    names = [n for p in glob.glob(os.path.join(WORKLIST_DIR, "pack_*.zip")) for n in zipfile.ZipFile(p).namelist()]
+    return sorted(os.path.join(ROOT, "tests", "golden", "streams", n[:-7] + ".hevc") for n in names if n.count(".") == 2)

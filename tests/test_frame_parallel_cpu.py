@@ -100,6 +100,41 @@ def test_two_rank_frame_parallel_equals_sequential():
     assert not bad, bad
 
 
+@pytest.mark.parametrize("n_gops", [1, 5, 8, 11])
+def test_schedule_decodes_exactly_the_requested_gops(n_gops):
+    """one rank: n_gops GOPs of 8 pictures, also when n_gops is no multiple of the intra period; every reference written first"""
+    class Record:
+        def __init__(self):
+            self.pics, self.written = [], {FP.anchor_slot(-1)}
+
+        def decode(self, pic, g=None):
+            assert all(r in self.written for r in pic.ref_slots), (g, pic)
+            self.written.add(pic.cur_slot)
+            self.pics.append((g, pic))
+
+        def exchange_anchors(self, *a):
+            pass
+    rec = Record()
+    assert FP.run_schedule(rec, 0, 1, n_gops) == 8 * n_gops == len(rec.pics)
+    assert sorted({g for g, _ in rec.pics}) == list(range(n_gops))
+
+
+def test_schedule_with_several_ranks_decodes_a_prefix_of_the_stream():
+    """two ranks, 5 GOPs asked: whole intra periods (8 GOPs per rank), GOPs 0..15 and nothing else"""
+    class Record:
+        def __init__(self):
+            self.gops = set()
+
+        def decode(self, pic, g=None):
+            self.gops.add(g)
+
+        def exchange_anchors(self, *a):
+            pass
+    recs = [Record(), Record()]
+    assert [FP.run_schedule(r, rank, 2, 5) for rank, r in enumerate(recs)] == [64, 64]
+    assert sorted(recs[0].gops | recs[1].gops) == list(range(16))
+
+
 def test_gop_plan_is_consistent():
     for g in range(40):
         pics = FP.gop_pictures(g)

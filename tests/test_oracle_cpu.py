@@ -107,7 +107,7 @@ def test_table_level_library_exports_every_declared_symbol(built):
     declared = set(re.findall(r"\b((?:ff_hevcdsp|ff_hevcpred|ff_videodsp)_init_b200|b200_[a-z0-9_]+)\s*\(", hdr))
     assert {"ff_hevcdsp_init_b200", "ff_hevcpred_init_b200", "ff_videodsp_init_b200", "b200_frame_begin", "b200_frame_end",
             "b200_frame_readback", "b200_frame_fill", "b200_host_pixels_unused"} <= declared
-    path = os.path.join(oracle_lib.ROOT, "openhevc_b200", "libb200hevc_shim.so")
+    path = oracle_lib.SHIM_SO
     if not os.path.exists(path):
         pytest.skip("libb200hevc_shim.so not built (needs the reference headers)")
     lib = ctypes.CDLL(path)

@@ -2,8 +2,8 @@
 """timeline.py — reads the CSV written by B200_TRACE=<file> (engine.cu: events at the stage boundaries of every picture as
 it really ran on its compute lane) and answers what per-kernel tools cannot: how well the pictures overlap.
 
-    B200_TRACE=gpurun_out/trace.csv python bench.py --steps 16 --warmup 3 --no-cpu-baseline
-    python tools/timeline.py gpurun_out/trace.csv [--from 64]
+    B200_TRACE=/tmp/trace.csv python bench.py --steps 16 --warmup 3 --no-cpu-baseline
+    python tools/timeline.py /tmp/trace.csv [--from 64]
 
 Prints per-picture stage times under load, the number of pictures in flight over time, the busy fraction of every lane
 and the critical-path / throughput bounds of the run.
