@@ -37,8 +37,8 @@ typedef struct B200Rec B200Rec;
 /* Threading contract.  A B200Ctx is driven by ONE submitting thread at a time: every call that takes a B200Ctx and is not
  * listed below mutates un-locked context state (slot hazards, arenas, lanes) and must come from that thread, pictures in
  * decode order (the table-level shim runs a dedicated submission thread for exactly this reason).  Callable from ANY
- * thread, concurrently with the submitting thread: b200_upload_wait, b200_readback_wait (they touch an immutable event
- * handle only), b200_last_error, the b200_host_* functions and every b200_rec_* function (a B200Rec belongs to the thread
+ * thread, concurrently with the submitting thread: b200_upload_wait, b200_readback_wait, b200_export_wait,
+ * b200_export_event (they touch an immutable event handle only), b200_yuv_to_rgb (no context), b200_last_error, the b200_host_* functions and every b200_rec_* function (a B200Rec belongs to the thread
  * that records into it).  b200_ctx_create / b200_ctx_destroy are serialised internally. */
 
 typedef struct B200Config {
@@ -102,6 +102,43 @@ int b200_slot_readback(B200Ctx *ctx, int slot, void *const planes[3], const int6
  * after it was decoded): asynchronous like b200_slot_readback, *token names its completion for b200_readback_wait */
 int b200_slot_readback_async(B200Ctx *ctx, int slot, void *const planes[3], const int64_t strides[3], uint32_t *token);
 int b200_readback_wait(B200Ctx *ctx, uint32_t token);        /* any thread; host blocks until that read-back has landed */
+/* ---- device-resident output ----------------------------------------------------------------------
+ * b200_slot_export_async copies one DPB slot into caller-owned DEVICE memory, in the same AVFrame layout (uint8 samples at 8
+ * bit, uint16 above), optionally cropped.  The copy is a reader of the slot like a read-back: it starts after the slot's last
+ * writer, and a later picture that writes the slot waits for it.  *token names its completion: b200_export_wait blocks the
+ * host, b200_export_event returns the cudaEvent_t (as void *) that a consumer's stream can wait on instead.  Tokens are
+ * recycled after 64 further exports; both calls may come from any thread. */
+typedef struct B200Export {
+    void    *planes[3];         /* device destinations: Y, Cb, Cr                                                            */
+    int64_t  pitches[3];        /* bytes per row                                                                            */
+    int32_t  crop_x, crop_y;    /* crop window in luma samples; chroma offsets follow the chroma format, so x / width must   */
+    int32_t  crop_w, crop_h;    /*   be even unless 4:4:4 and y / height even for 4:2:0.  crop_w == crop_h == 0: whole picture */
+    void    *after_event;       /* optional cudaEvent_t: the copy starts after it (e.g. the destination's previous consumer)  */
+} B200Export;
+int   b200_slot_export_async(B200Ctx *ctx, int slot, const B200Export *e, uint32_t *token);
+int   b200_export_wait(B200Ctx *ctx, uint32_t token);         /* any thread; host blocks until that export has landed */
+void *b200_export_event(B200Ctx *ctx, uint32_t token);        /* any thread; cudaEvent_t of that export, NULL for a bad token */
+
+/* YUV (AVFrame layout, device memory: a DPB slot, an export target, ...) -> planar RGB (CHW, contiguous) in caller device
+ * memory, as uint8 or as float32 in [0, 1], on `stream` (a cudaStream_t; NULL = the legacy default stream).  The matrix and
+ * the range are the caller's: the decoder does not read the VUI colour description.  Chroma is upsampled by nearest sample.
+ * The fixed-point definition of the arithmetic is in openhevc_b200/csrc/k_yuv_rgb.cuh.  B200_ENOTSUP for a matrix, chroma
+ * format or bit depth outside the list below. */
+typedef struct B200RgbArgs {
+    const void *planes[3];      /* device Y, Cb, Cr                                                                          */
+    int64_t     pitches[3];     /* bytes per row                                                                             */
+    int32_t     width, height;  /* luma samples of the planes                                                                */
+    int32_t     chroma_format_idc;  /* 1 = 4:2:0, 2 = 4:2:2, 3 = 4:4:4                                                       */
+    int32_t     bit_depth;      /* 8..12                                                                                     */
+    int32_t     crop_x, crop_y, crop_w, crop_h;   /* luma samples, any offsets and sizes; crop_w == crop_h == 0: whole picture  */
+    int32_t     matrix;         /* matrix_coefficients: 1 = BT.709, 5 or 6 = BT.601, 9 = BT.2020 non-constant luminance       */
+    int32_t     full_range;     /* 0 = limited (video) range, 1 = full range                                                 */
+    int32_t     out_float;      /* 0 = uint8, 1 = float32                                                                    */
+    int32_t     reserved0;
+    void       *out;            /* 3 x crop_h x crop_w samples: R, G, B planes                                               */
+} B200RgbArgs;
+int b200_yuv_to_rgb(const B200RgbArgs *a, void *stream);
+
 int b200_poll_errors(B200Ctx *ctx);                          /* device-side error latches (rejected work list, intra dependency time-out)
                                                                 WITHOUT synchronising: 0 or the error b200_sync would report */
 int b200_slot_wait_readback(B200Ctx *ctx, int slot);         /* host blocks until the slot's last read-back has landed (not for the whole queue) */

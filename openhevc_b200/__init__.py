@@ -6,4 +6,5 @@ Python package is a thin host-side mirror used by tests and bench.py: it never c
 itself and has no CPU fallback.
 """
 from .engine import FrameEngine, B200Error  # noqa: F401
+from .device_output import yuv_to_rgb  # noqa: F401
 from . import worklist  # noqa: F401

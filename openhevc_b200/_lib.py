@@ -14,13 +14,25 @@ class B200Config(C.Structure):
                 ("n_lanes", C.c_int32), ("reserved0", C.c_int32)]
 
 
+class B200Export(C.Structure):
+    _fields_ = [("planes", C.c_void_p * 3), ("pitches", C.c_int64 * 3), ("crop_x", C.c_int32), ("crop_y", C.c_int32),
+                ("crop_w", C.c_int32), ("crop_h", C.c_int32), ("after_event", C.c_void_p)]
+
+
+class B200RgbArgs(C.Structure):
+    _fields_ = [("planes", C.c_void_p * 3), ("pitches", C.c_int64 * 3), ("width", C.c_int32), ("height", C.c_int32),
+                ("chroma_format_idc", C.c_int32), ("bit_depth", C.c_int32), ("crop_x", C.c_int32), ("crop_y", C.c_int32),
+                ("crop_w", C.c_int32), ("crop_h", C.c_int32), ("matrix", C.c_int32), ("full_range", C.c_int32),
+                ("out_float", C.c_int32), ("reserved0", C.c_int32), ("out", C.c_void_p)]
+
+
 EXPORTS = [  # every symbol include/b200hevc.h declares
     "b200_ctx_create", "b200_ctx_destroy", "b200_last_error", "b200_dpb_bytes", "b200_slot_bytes", "b200_slot_devptr",
     "b200_stream", "b200_join", "b200_slot_begin_access", "b200_slot_end_access", "b200_host_alloc", "b200_host_free", "b200_frame_upload", "b200_frame_execute", "b200_frame_execute_ex", "b200_frame_submit",
     "b200_slot_upload", "b200_slot_readback", "b200_slot_wait_readback", "b200_slot_fill", "b200_wait_uploads", "b200_sync", "b200_set_profiling", "b200_get_stage_ms",
     "b200_launch_count", "b200_rec_create", "b200_rec_destroy", "b200_rec_begin", "b200_rec_set_refs", "b200_rec_tu", "b200_rec_pcm",
     "b200_host_register", "b200_host_unregister", "b200_frame_submit_ex", "b200_upload_wait", "b200_slot_readback_async", "b200_readback_wait", "b200_poll_errors",
-    "b200_rec_bs_leaf", "b200_rec_set_dbd",
+    "b200_rec_bs_leaf", "b200_rec_set_dbd", "b200_slot_export_async", "b200_export_wait", "b200_export_event", "b200_yuv_to_rgb",
     "b200_rec_intra", "b200_rec_mc", "b200_rec_deblock", "b200_rec_sao", "b200_rec_set_cip", "b200_rec_set_tqb", "b200_rec_tu_parked", "b200_rec_ccp", "b200_rec_merge", "b200_rec_finish", "b200_intra_level_order", "b200_intra_ctb_order",
 ]
 
@@ -48,6 +60,10 @@ def load():
         "b200_slot_readback_async": (i32, [vp, i32, C.POINTER(vp), C.POINTER(i64), C.POINTER(C.c_uint32)]),
         "b200_readback_wait": (i32, [vp, C.c_uint32]),
         "b200_poll_errors": (i32, [vp]),
+        "b200_slot_export_async": (i32, [vp, i32, C.POINTER(B200Export), C.POINTER(C.c_uint32)]),
+        "b200_export_wait": (i32, [vp, C.c_uint32]),
+        "b200_export_event": (vp, [vp, C.c_uint32]),
+        "b200_yuv_to_rgb": (i32, [C.POINTER(B200RgbArgs), vp]),
         "b200_join": (i32, [vp]),
         "b200_slot_begin_access": (i32, [vp, i32, vp, i32]),
         "b200_slot_end_access": (i32, [vp, i32, vp, i32]),

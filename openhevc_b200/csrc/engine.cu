@@ -24,13 +24,17 @@
 #include <vector>
 #include "../../include/b200hevc.h"
 #include "common.cuh"
+#include "k_yuv_rgb.cuh"
+
+int launch_yuv_rgb(cudaStream_t st, const YuvRgbJob &j, int bd, int out_float);     // kernels.cu
 
 #define MAX_SLOTS 64
 #define MAX_ARENAS 16
 #define MAX_LANES 16
 #define RD_DOWN MAX_LANES            // reader index of the read-back stream
 #define RD_EXT (MAX_LANES + 1)       // reader index of caller-owned streams (b200_slot_end_access)
-#define N_RD (MAX_LANES + 2)
+#define RD_EXP (MAX_LANES + 2)       // reader index of the export stream (b200_slot_export_async)
+#define N_RD (MAX_LANES + 3)
 #define RB_RING 64
 
 struct Arena {
@@ -93,6 +97,10 @@ struct B200Ctx {
     // read-backs whose completion other threads wait for (b200_readback_wait): a ring of events on the read-back stream
     cudaEvent_t rb_ev[RB_RING] = {};
     uint32_t rb_next = 0;
+    // device-to-device exports (b200_slot_export_async): their own stream, so that they do not queue behind host read-backs
+    cudaStream_t st_exp = nullptr;
+    cudaEvent_t ex_ev[RB_RING] = {};
+    uint32_t ex_next = 0;
     // device-side error latches mirrored in mapped host memory (one word per lane): readable without a synchronisation
     volatile uint32_t *err_host = nullptr;
     uint32_t *err_dev = nullptr;
@@ -263,6 +271,7 @@ extern "C" void b200_ctx_destroy(B200Ctx *ctx)
     }
     for (int i = 0; i <= B200_ST_COUNT; i++) if (ctx->prof[i]) cudaEventDestroy(ctx->prof[i]);
     for (int i = 0; i < RB_RING; i++) if (ctx->rb_ev[i]) cudaEventDestroy(ctx->rb_ev[i]);
+    for (int i = 0; i < RB_RING; i++) if (ctx->ex_ev[i]) cudaEventDestroy(ctx->ex_ev[i]);
     if (ctx->err_host) cudaFreeHost((void *)ctx->err_host);
     if (ctx->own_dpb && ctx->dpb) cudaFree(ctx->dpb);
     if (ctx->dpb_desc_dev) cudaFree(ctx->dpb_desc_dev);
@@ -280,6 +289,7 @@ extern "C" void b200_ctx_destroy(B200Ctx *ctx)
     }
     if (ctx->st_copy) cudaStreamDestroy(ctx->st_copy);
     if (ctx->st_down) cudaStreamDestroy(ctx->st_down);
+    if (ctx->st_exp) cudaStreamDestroy(ctx->st_exp);
     delete ctx;
 }
 
@@ -333,6 +343,7 @@ static int ctx_init(B200Ctx *ctx)
         ctx->err_dev = (uint32_t *)ed;
     }
     for (int i = 0; i < RB_RING; i++) CU(cudaEventCreateWithFlags(&ctx->rb_ev[i], cudaEventDisableTiming));
+    for (int i = 0; i < RB_RING; i++) CU(cudaEventCreateWithFlags(&ctx->ex_ev[i], cudaEventDisableTiming));
     for (int l = 0; l < ctx->n_lanes; l++) {
         Lane &L = ctx->lane[l];
         CU(cudaStreamCreateWithFlags(&L.st, cudaStreamNonBlocking));
@@ -356,6 +367,7 @@ static int ctx_init(B200Ctx *ctx)
     ctx->st_compute = ctx->lane[0].st;
     CU(cudaStreamCreateWithFlags(&ctx->st_copy, cudaStreamNonBlocking));
     CU(cudaStreamCreateWithFlags(&ctx->st_down, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&ctx->st_exp, cudaStreamNonBlocking));
     for (int i = 0; i < c.n_arenas; i++) {
         CU(cudaMalloc(&ctx->arena[i].dev, ctx->arena_bytes));
         CU(cudaEventCreateWithFlags(&ctx->arena[i].ev_uploaded, cudaEventDisableTiming));
@@ -829,6 +841,92 @@ extern "C" int b200_readback_wait(B200Ctx *ctx, uint32_t token)
     return e == cudaSuccess ? 0 : B200_ECUDA;
 }
 
+// device-to-device copy of one slot (cropped) into caller memory: a reader of the slot on the export stream, completion named
+// by a ring of events like the read-backs
+extern "C" int b200_slot_export_async(B200Ctx *ctx, int slot, const B200Export *e, uint32_t *token)
+{
+    if (!ctx || slot < 0 || slot >= ctx->cfg.n_slots || !e) return B200_EINVAL;
+    if (ctx->err_code) return ctx->err_code;
+    const int sx = ctx->cfg.chroma_format_idc != 3, sy = ctx->cfg.chroma_format_idc == 1;
+    int x = e->crop_x, y = e->crop_y, w = e->crop_w, h = e->crop_h;
+    if (!w && !h) { x = 0; y = 0; w = ctx->cfg.width; h = ctx->cfg.height; }
+    const int B = ctx->cfg.bit_depth > 8 ? 2 : 1;
+    // argument errors are reported, not latched: the context stays usable
+    int rc = 0;
+    if (x < 0 || y < 0 || w <= 0 || h <= 0 || (int64_t)x + w > ctx->cfg.width || (int64_t)y + h > ctx->cfg.height || ((x | w) & sx) || ((y | h) & sy))
+        rc = fail(ctx, B200_EINVAL, "export crop window %d,%d %dx%d does not fit the %dx%d picture / its chroma grid", x, y, w, h, ctx->cfg.width, ctx->cfg.height);
+    for (int p = 0; p < 3 && !rc; p++) {
+        const int64_t row = (int64_t)(w >> (p ? sx : 0)) * B;
+        if (!e->planes[p]) rc = fail(ctx, B200_EINVAL, "export plane %d is NULL", p);
+        else if (e->pitches[p] < row) rc = fail(ctx, B200_EINVAL, "export plane %d: pitch %lld < %lld bytes per row", p, (long long)e->pitches[p], (long long)row);
+    }
+    if (rc) { ctx->err_code = 0; return rc; }
+    CU(cudaSetDevice(ctx->cfg.device));
+    if (e->after_event && cudaStreamWaitEvent(ctx->st_exp, (cudaEvent_t)e->after_event, 0) != cudaSuccess) {
+        cudaGetLastError();
+        rc = fail(ctx, B200_EINVAL, "export: after_event is not a valid CUDA event of this device");
+        ctx->err_code = 0;
+        return rc;
+    }
+    if ((rc = slot_acquire(ctx, slot, ctx->st_exp, RD_EXP, false))) return rc;
+    cudaError_t ce = cudaSuccess;
+    for (int p = 0; p < 3 && ce == cudaSuccess; p++) {
+        const int hs = p ? sx : 0, vs = p ? sy : 0;
+        const PlaneDesc &d = ctx->slot_desc[slot].p[p];
+        ce = cudaMemcpy2DAsync(e->planes[p], (size_t)e->pitches[p], d.base + (size_t)(y >> vs) * d.pitch + (size_t)(x >> hs) * B, d.pitch,
+                               (size_t)(w >> hs) * B, (size_t)(h >> vs), cudaMemcpyDeviceToDevice, ctx->st_exp);
+    }
+    // the reader is published even when a copy failed to enqueue: a later writer of the slot must not skip what was queued
+    if ((rc = slot_release(ctx, slot, ctx->st_exp, RD_EXP, false))) return rc;
+    if (ce != cudaSuccess) return fail(ctx, B200_ECUDA, "export copy: %s", cudaGetErrorString(ce));
+    const uint32_t i = ctx->ex_next;
+    ctx->ex_next = (i + 1) % RB_RING;
+    CU(cudaEventRecord(ctx->ex_ev[i], ctx->st_exp));
+    if (token) *token = i;
+    return 0;
+}
+extern "C" int b200_export_wait(B200Ctx *ctx, uint32_t token)
+{
+    if (!ctx || token >= RB_RING) return B200_EINVAL;
+    cudaSetDevice(ctx->cfg.device);
+    const cudaError_t e = cudaEventSynchronize(ctx->ex_ev[token]);
+    return e == cudaSuccess ? 0 : B200_ECUDA;
+}
+extern "C" void *b200_export_event(B200Ctx *ctx, uint32_t token)
+{
+    return ctx && token < RB_RING ? (void *)ctx->ex_ev[token] : nullptr;
+}
+
+extern "C" int b200_yuv_to_rgb(const B200RgbArgs *a, void *stream)
+{
+    if (!a) return B200_EINVAL;
+    YuvRgbJob j;
+    if (a->chroma_format_idc < 1 || a->chroma_format_idc > 3 || a->bit_depth < 8 || a->bit_depth > 12 || (a->out_float != 0 && a->out_float != 1) ||
+        !yuv_rgb_coef(a->matrix, a->full_range != 0, a->bit_depth, a->out_float, &j.k))
+        return B200_ENOTSUP;
+    j.sx = a->chroma_format_idc != 3; j.sy = a->chroma_format_idc == 1;
+    j.x0 = a->crop_x; j.y0 = a->crop_y; j.w = a->crop_w; j.h = a->crop_h;
+    if (!j.w && !j.h) { j.x0 = 0; j.y0 = 0; j.w = a->width; j.h = a->height; }
+    if (a->width <= 0 || a->height <= 0 || j.x0 < 0 || j.y0 < 0 || j.w <= 0 || j.h <= 0 || (int64_t)j.x0 + j.w > a->width || (int64_t)j.y0 + j.h > a->height || !a->out)
+        return B200_EINVAL;
+    const int B = a->bit_depth > 8 ? 2 : 1;
+    for (int p = 0; p < 3; p++) {
+        const int pw = p ? (a->width + j.sx) >> j.sx : a->width;
+        if (!a->planes[p] || a->pitches[p] < (int64_t)pw * B) return B200_EINVAL;
+        j.src[p] = (const uint8_t *)a->planes[p];
+        j.pitch[p] = a->pitches[p];
+    }
+    j.tx0 = j.x0 >> 1; j.ty0 = j.y0 >> 1;
+    j.dst = a->out;
+    // The library links its own (static) CUDA runtime, so this thread's last-error state holds errors of this library only,
+    // never those of the caller's runtime (torch ...).  Every other b200_* call checks its CUDA calls as it makes them and
+    // returns what failed, so an error still pending here was reported already.  Clear it, so that the check after the launch
+    // reports the launch alone.
+    cudaGetLastError();
+    launch_yuv_rgb((cudaStream_t)stream, j, a->bit_depth, a->out_float);
+    return cudaGetLastError() == cudaSuccess ? 0 : B200_ECUDA;
+}
+
 // Device-side error latches without a synchronisation: the kernels mirror them into mapped host memory (one word per lane)
 extern "C" int b200_poll_errors(B200Ctx *ctx)
 {
@@ -893,6 +991,7 @@ extern "C" int b200_sync(B200Ctx *ctx)
     CU(cudaStreamSynchronize(ctx->st_copy));
     for (int l = 0; l < ctx->n_lanes; l++) CU(cudaStreamSynchronize(ctx->lane[l].st));
     CU(cudaStreamSynchronize(ctx->st_down));
+    CU(cudaStreamSynchronize(ctx->st_exp));
     for (int l = 0; l < ctx->n_lanes; l++) {
         if (!ctx->lane[l].used) continue;
         uint32_t st[4] = { 0, 0, 0, 0 };

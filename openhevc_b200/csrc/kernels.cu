@@ -1784,3 +1784,25 @@ int launch_fill(cudaStream_t st, const FrameDesc &f, int bd, int value)
     else        B200_LAUNCH(g, 256, 0, st, k_fill<uint8_t>)(f, value);
     return 1;
 }
+
+// --------------------------------------------------------------------------------------------
+// YUV -> planar RGB for consumers on the device (b200_yuv_to_rgb): one thread per 2x2 luma tile, a warp covers 64 consecutive
+// samples of two rows, so loads and stores of a warp are contiguous runs
+#include "k_yuv_rgb.cuh"
+
+template <typename PIX, typename OUT>
+__global__ void __launch_bounds__(256) k_yuv_rgb(YuvRgbJob j, int nx, int ny)
+{
+    const int tx = blockIdx.x * blockDim.x + threadIdx.x, ty = blockIdx.y * blockDim.y + threadIdx.y;
+    if (tx >= nx || ty >= ny) return;
+    yuv_rgb_tile<PIX, OUT>(j, j.tx0 + tx, j.ty0 + ty);
+}
+
+int launch_yuv_rgb(cudaStream_t st, const YuvRgbJob &j, int bd, int out_float)
+{
+    const int nx = ((j.x0 + j.w - 1) >> 1) - j.tx0 + 1, ny = ((j.y0 + j.h - 1) >> 1) - j.ty0 + 1;
+    const dim3 g((nx + 31) / 32, (ny + 7) / 8), b(32, 8);
+    if (bd > 8) { if (out_float) B200_LAUNCH(g, b, 0, st, k_yuv_rgb<uint16_t, float>)(j, nx, ny); else B200_LAUNCH(g, b, 0, st, k_yuv_rgb<uint16_t, uint8_t>)(j, nx, ny); }
+    else        { if (out_float) B200_LAUNCH(g, b, 0, st, k_yuv_rgb<uint8_t, float>)(j, nx, ny);  else B200_LAUNCH(g, b, 0, st, k_yuv_rgb<uint8_t, uint8_t>)(j, nx, ny); }
+    return 1;
+}

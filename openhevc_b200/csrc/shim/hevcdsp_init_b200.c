@@ -78,8 +78,9 @@ typedef struct Instance {
     pthread_cond_t cv_sub;
     int sub_running, sub_stop;
     int err_code; char errmsg[256];     /* latched by the submission thread, returned by the next b200_frame_begin / _end */
-    /* read-backs in flight, keyed by the host frame's luma pointer (b200_output_wait) */
-    struct { const uint8_t *data0; uint32_t token; int state; unsigned seq; } rb[MAX_RB];
+    /* read-backs in flight, keyed by the host frame's luma buffer [data0, end) (b200_output_wait): an output frame with a
+     * conformance window points inside it (ff_hevc_output_frame moves the data pointers by the window's offsets) */
+    struct { const uint8_t *data0, *end; uint32_t token; int state; unsigned seq; } rb[MAX_RB];
     unsigned rb_seq;
     uint64_t n_pictures, h2d_bytes, d2h_bytes;   /* B200_SHIM_REPORT=1: totals on stderr when the process ends */
     uint64_t ns_ctx, ns_rec, ns_pool, n_pool, bytes_pool, ns_first_submit;   /* ... and where the start-up time went */
@@ -905,7 +906,7 @@ static void deactivate(void)                       /* the picture is no longer o
 
 static void finish_abandoned(HEVCContext *s);
 static void picture_flags(HEVCContext *s);
-static int rb_insert(const uint8_t *data0);
+static int rb_insert(const uint8_t *data0, size_t luma_bytes);
 
 int b200_frame_begin(HEVCContext *s)
 {
@@ -967,13 +968,13 @@ int b200_frame_begin(HEVCContext *s)
     /* announce the read-back NOW: the frame may be picked for output (bumping, by the thread of a later picture) while this
      * thread is still parsing it, and whoever hands it to the application must wait for pixels that are not even queued yet */
     g.rb_at = -1;
-    if (!G.dump_dir && s->frame->data[0]) { g.rb_at = rb_insert(s->frame->data[0]); if (g.rb_at >= 0) g.rb_seq = G.rb[g.rb_at].seq; }
+    if (!G.dump_dir && s->frame->data[0]) { g.rb_at = rb_insert(s->frame->data[0], (size_t)s->frame->linesize[0] * s->sps->height); if (g.rb_at >= 0) g.rb_seq = G.rb[g.rb_at].seq; }
     pthread_mutex_unlock(&G.mu);
     return 0;
 }
 
 /* a read-back into `data0`'s frame is on its way: remembered until the frame leaves the decoder (b200_output_wait).  G.mu held. */
-static int rb_insert(const uint8_t *data0)
+static int rb_insert(const uint8_t *data0, size_t luma_bytes)
 {
     int at = -1, oldest = -1;
     for (int i = 0; i < MAX_RB; i++) {
@@ -983,7 +984,7 @@ static int rb_insert(const uint8_t *data0)
     }
     if (at < 0) at = oldest;                       /* table full of pictures nobody asked for: forget the oldest one */
     if (at < 0) return -1;
-    G.rb[at].data0 = data0; G.rb[at].state = 1; G.rb[at].seq = G.rb_seq++; G.rb[at].token = 0;
+    G.rb[at].data0 = data0; G.rb[at].end = data0 + luma_bytes; G.rb[at].state = 1; G.rb[at].seq = G.rb_seq++; G.rb[at].token = 0;
     return at;
 }
 
@@ -1100,7 +1101,8 @@ int b200_output_wait(HEVCContext *s, AVFrame *frame)
     if (!frame || !frame->data[0] || G.dump_dir) return 0;
     pthread_mutex_lock(&G.mu);
     int at = -1;
-    for (int i = 0; i < MAX_RB; i++) if (G.rb[i].state && G.rb[i].data0 == frame->data[0]) { at = i; break; }
+    for (int i = 0; i < MAX_RB; i++)                /* the frame's luma pointer lies inside the buffer (cropped frames: past its start) */
+        if (G.rb[i].state && G.rb[i].data0 <= frame->data[0] && frame->data[0] < G.rb[i].end) { at = i; break; }
     if (at < 0) { pthread_mutex_unlock(&G.mu); return 0; }
     const unsigned seq = G.rb[at].seq;
     while (G.rb[at].state == 1 && G.rb[at].seq == seq && !G.err_code) pthread_cond_wait(&G.cv, &G.mu);

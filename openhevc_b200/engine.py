@@ -8,7 +8,7 @@ accepts one work-list blob per picture and hands planes back in the reference's 
 import ctypes as C
 import numpy as np
 
-from . import _lib
+from . import _lib, device_output
 from .worklist import plane_dims
 
 STAGES = ("mc", "residual", "intra", "deblock", "sao", "total")
@@ -123,6 +123,12 @@ class FrameEngine:
         if sync:
             self.sync()
         return out
+
+    def export(self, slot, out=None, crop=None, stream=None):
+        """the picture in DPB slot `slot` as three torch CUDA tensors (H, W): uint8 at 8 bit, int16 above; crop = (x, y, w, h)
+        in luma samples.  Ordered on `stream` (default: torch's current stream) after the slot's last writer; a later picture
+        that rewrites the slot waits for the copy.  No host synchronisation."""
+        return device_output.export(self, slot, out, crop, stream)
 
     def wait_readback(self, slot):
         """block until the last read-back of `slot` has landed in host memory (the queue keeps running)"""

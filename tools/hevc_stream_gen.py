@@ -233,6 +233,7 @@ class StreamGen:
     def __init__(self, width, height, bit_depth=8, seed=1, qp=30, sao=True, ctb_log2=6, weighted=False, wpp=False, cip=False, tqb=0.0, tiles=None, lf_across_tiles=True, tskip=0.0, pcm=0.0, pcm_lf_off=False, slices=1, lf_across_slices=True, cfi=1, calm=0.0, ccp=False, amp=False, qpd=False, dbk_offsets=(0, 0), chroma_qp_offsets=(0, 0), tmvp=False, no_dbk=False, sao_planes="both"):
         self.W, self.H, self.bd, self.qp, self.sao, self.ctb_log2 = width, height, bit_depth, qp, sao, ctb_log2
         self.weighted = weighted
+        self.conf_win = None                # (L, R, T, B) luma samples of the SPS conformance window, None = flag 0
         self.cip = cip                      # pps constrained_intra_pred_flag (hevcpred_template.c:116-249)
         self.tqb = tqb                      # share of CUs with cu_transquant_bypass_flag (pps transquant_bypass_enable_flag when > 0)
         self.cfi = cfi                      # chroma_format_idc: 1 = 4:2:0, 2 = 4:2:2 (two stacked chroma blocks per TU, RExt), 3 = 4:4:4 (chroma like luma, RExt)
@@ -301,7 +302,13 @@ class StreamGen:
         if self.cfi == 3:
             w.u(1, 0)                                                      # separate_colour_plane_flag (hevc_ps.c:1597)
         w.ue(self.W); w.ue(self.H)
-        w.u(1, 0)                                                          # conformance window
+        if self.conf_win:                                                  # conformance window: offsets in chroma sample units
+            sw, sh = (1 if self.cfi == 3 else 2), (2 if self.cfi == 1 else 1)
+            w.u(1, 1)
+            for v, unit in zip(self.conf_win, (sw, sw, sh, sh)):
+                w.ue(v // unit)
+        else:
+            w.u(1, 0)
         w.ue(self.bd - 8); w.ue(self.bd - 8)
         w.ue(4)                                                            # log2_max_poc_lsb - 4
         w.u(1, 1); w.ue(4); w.ue(self.reorder); w.ue(0)                   # sub_layer_ordering_info: dpb 5, num_reorder, latency
@@ -1134,11 +1141,16 @@ def main():
     ap.add_argument("--amp", action="store_true", help="amp_enabled_flag: asymmetric motion partitions")
     ap.add_argument("--ccp", action="store_true", help="cross_component_prediction_enabled_flag (needs --cfi 3)")
     ap.add_argument("--calm", type=float, default=0.0, help="0 = dense random content (default) .. 1 = lightly coded (more skip, larger CUs, sparse residuals)")
+    ap.add_argument("--conf-win", default="", help="L,R,T,B: conformance window offsets in luma samples (multiples of the chroma subsampling)")
     ap.add_argument("--wpp", action="store_true", help="entropy_coding_sync_enabled_flag: one substream per CTB row + entry points")
     a = ap.parse_args()
     verify_tables_against_reference()
     g = StreamGen(a.width, a.height, a.bit_depth, a.seed, a.qp, sao=not a.no_sao, weighted=a.weighted, wpp=a.wpp, cip=a.cip, tqb=a.tqb, tskip=a.tskip, pcm=a.pcm, pcm_lf_off=a.pcm_lf_off, slices=a.slices, lf_across_slices=not a.no_lf_across_slices, cfi=a.cfi, calm=a.calm, ccp=a.ccp, amp=a.amp, qpd=a.qpd, tmvp=a.tmvp, no_dbk=a.no_dbk, sao_planes=a.sao_planes, dbk_offsets=tuple(int(v) for v in a.dbk_offsets.split(",")), chroma_qp_offsets=tuple(int(v) for v in a.chroma_qp_offsets.split(",")),
                   tiles=tuple(int(v) for v in a.tiles.split("x")) if a.tiles else None, lf_across_tiles=not a.no_lf_across_tiles)
+    if a.conf_win:
+        g.conf_win = tuple(int(v) for v in a.conf_win.split(","))
+        sw, sh = (1 if a.cfi == 3 else 2), (2 if a.cfi == 1 else 1)
+        assert len(g.conf_win) == 4 and all(v >= 0 for v in g.conf_win) and not (g.conf_win[0] | g.conf_win[1]) % sw and not (g.conf_win[2] | g.conf_win[3]) % sh
     data = g.stream(a.frames, a.pattern)
     open(a.out, "wb").write(data)
     print(f"wrote {a.out}: {len(data)} bytes, {a.frames} pictures {a.width}x{a.height} {a.bit_depth}-bit")
