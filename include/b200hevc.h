@@ -203,11 +203,6 @@ int  b200_rec_set_dbd(B200Rec *r, const B200DbdInput *in);
 /* host helper shared by the recorder and by external blob builders: permutation (perm[new] = old) that sorts decode-order
  * intra records by dependency level (stable); returns the number of levels (>= 0) or a negative error */
 int  b200_intra_level_order(const B200IntraRec *recs, uint32_t n, int width, int height, int chroma_format_idc, uint32_t *perm);
-/* the order of the CTB-granular intra stage: records grouped by CTB (raster order), inside a CTB by the dependency level counted
- * inside the CTB; perm[new] = old, ctb_start[ctb_count + 1] (B200BlobHeader.ictb), level[new] (B200IntraRec.pad[0]); returns the
- * largest level or a negative error (B200_ENOTSUP: more than 255 levels, use the picture-wide order) */
-int  b200_intra_ctb_order(const B200IntraRec *recs, uint32_t n, int width, int height, int chroma_format_idc, int log2_ctb_size,
-                          uint32_t *perm, uint32_t *ctb_start, uint8_t *level);
 /* finish: returns the blob (pinned memory owned by the recorder, valid until the next begin) */
 int b200_rec_merge(B200Rec *dst, B200Rec *src);           /* fold the lists of a worker thread of the SAME picture into dst (WPP / tiles / slices) */
 int  b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes);

@@ -77,10 +77,8 @@ typedef struct B200BlobHeader {
                                     reference's own per-edge calls, recorded) or this section (its inputs: transform-tree leaves,
                                     QP map, per-CTB offsets; motion and cbf come from the MC / TU records), never both -- except in
                                     check mode (B200_DBD_CHECK), where the device compares what it derived with the recorded grids */
-    B200Section ictb;            /* CTB-granular intra stage (else count = 0): uint32[ctb_count + 1], records [ictb[c], ictb[c + 1]) of B200_SEC_INTRA
-                                    belong to CTB c (raster index); the list is then ordered by CTB and, inside a CTB, by the dependency
-                                    level counted inside the CTB (B200IntraRec.pad[0], 1 ..): b200_intra_ctb_order().  Without this section
-                                    the list is in picture-wide dependency-level order (b200_intra_level_order) */
+    B200Section reserved_section; /* off and count must both be zero (b200_frame_upload rejects the blob otherwise); holds the place of
+                                    the fields behind it */
     uint32_t mc_tile_count[5];   /* all zero: the records of B200_SEC_MC are TILES (<= 256 samples, ordered as mc_big_count says).  Else they are
                                     whole PREDICTION BLOCKS (w, h <= 64) in decode order and the DEVICE splits them (k_mc_expand): [0] tiles of
                                     any shape, [1 + B200_MC_SMALL_KEY] tiles of <= 8x8 samples; B200McRec.pad = index of the block's first
@@ -197,7 +195,7 @@ typedef struct B200IntraRec {    /* 16 bytes */
     uint8_t  flags;              /* B200_INF_* */
     uint8_t  top_right_size;     /* samples really inside the picture, hevcpred_template.c:108-109 */
     uint8_t  bottom_left_size;   /* hevcpred_template.c:106-107 */
-    uint8_t  pad[2];             /* pad[0]: dependency level inside the CTB when the blob carries B200BlobHeader.ictb */
+    uint8_t  pad[2];
     uint32_t resid_off;          /* int16 index of the parked residual in COEFF, 0xFFFFFFFF = cbf 0 */
 } B200IntraRec;
 #define B200_NO_RESID 0xFFFFFFFFu

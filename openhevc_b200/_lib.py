@@ -33,7 +33,7 @@ EXPORTS = [  # every symbol include/b200hevc.h declares
     "b200_launch_count", "b200_rec_create", "b200_rec_destroy", "b200_rec_begin", "b200_rec_set_refs", "b200_rec_tu", "b200_rec_pcm",
     "b200_host_register", "b200_host_unregister", "b200_frame_submit_ex", "b200_upload_wait", "b200_slot_readback_async", "b200_readback_wait", "b200_poll_errors",
     "b200_rec_bs_leaf", "b200_rec_set_dbd", "b200_slot_export_async", "b200_export_wait", "b200_export_event", "b200_yuv_to_rgb",
-    "b200_rec_intra", "b200_rec_mc", "b200_rec_deblock", "b200_rec_sao", "b200_rec_set_cip", "b200_rec_set_tqb", "b200_rec_tu_parked", "b200_rec_ccp", "b200_rec_merge", "b200_rec_finish", "b200_intra_level_order", "b200_intra_ctb_order",
+    "b200_rec_intra", "b200_rec_mc", "b200_rec_deblock", "b200_rec_sao", "b200_rec_set_cip", "b200_rec_set_tqb", "b200_rec_tu_parked", "b200_rec_ccp", "b200_rec_merge", "b200_rec_finish", "b200_intra_level_order",
 ]
 
 
@@ -99,7 +99,6 @@ def load():
         "b200_rec_merge": (i32, [vp, vp]),
         "b200_rec_finish": (i32, [vp, C.POINTER(vp), C.POINTER(u64)]),
         "b200_intra_level_order": (i32, [vp, C.c_uint32, i32, i32, i32, vp]),
-        "b200_intra_ctb_order": (i32, [vp, C.c_uint32, i32, i32, i32, i32, vp, vp, vp]),
     }
     for name in EXPORTS:
         fn = getattr(lib, name)          # AttributeError here == the .so does not export what the header declares

@@ -110,8 +110,6 @@ int launch_residual(cudaStream_t st, const B200TuRec *const recs[4], const int c
 int launch_ccp(cudaStream_t st, const B200CcpRec *recs, int count, int16_t *parked, const FrameDesc &cur, int bd, uint32_t *gate, unsigned long long arena_bytes);
 int launch_intra(cudaStream_t st, const B200IntraRec *recs, int count, const int16_t *pool, const FrameDesc &cur, int bd,
                  uint2 *edges[3], const int edge_stride[3], uint32_t *counter, const uint32_t *cip_words, const B200CipHeader *cip_hdr, int cfi);
-int launch_intra_ctb(cudaStream_t st, const B200IntraRec *recs, int count, const uint32_t *ctb_start, int ctb_w, int ctb_h, int log2_ctb, int cfi, const int16_t *parked,
-                     unsigned long long parked_cap, const FrameDesc &cur, int bd, uint32_t *counter, uint32_t *done, uint32_t gen);
 int launch_deblock(cudaStream_t st, const uint16_t *grid, const B200DbkLayout &L, const FrameDesc &cur, int bd);
 // on-device derivation of the deblocking parameters (k_dbd.cuh): per-lane scratch, one allocation starting at `mot`
 struct DbdMaps {

@@ -59,8 +59,6 @@ struct Lane {
     uint32_t *counter = nullptr;        // [0] K3 ticket, [1] validation gate of the picture in progress, [2] K3 time-out latch, [3] validation latch
     int16_t *parked = nullptr;          // residuals of intra TUs (K2 -> K3), indexed like the coefficient pool
     B200McRec *mc_tiles = nullptr;      // tile list k_mc_expand writes when the blob carries whole prediction blocks (B200BlobHeader.mc_tile_count)
-    uint32_t *ictb_done = nullptr;      // CTB-granular intra stage: one flag per CTB, == ictb_gen once the CTB of the picture in progress is done
-    uint32_t ictb_gen = 0;
     DbdMaps dbd = {};                   // scratch of the on-device deblocking derivation, allocated with the first picture that needs it
     size_t dbd_bytes = 0;
     cudaEvent_t tail = nullptr;         // end of the last picture of this lane
@@ -282,7 +280,6 @@ extern "C" void b200_ctx_destroy(B200Ctx *ctx)
         if (L.counter) cudaFree(L.counter);
         if (L.parked) cudaFree(L.parked);
         if (L.dbd.mot) cudaFree(L.dbd.mot);
-        if (L.ictb_done) cudaFree(L.ictb_done);
         if (L.mc_tiles) cudaFree(L.mc_tiles);
         if (L.tail) cudaEventDestroy(L.tail);
         if (L.st) cudaStreamDestroy(L.st);
@@ -445,10 +442,7 @@ static int check_blob(B200Ctx *ctx, const B200BlobHeader *h, uint64_t nbytes)
         if (!(h->flags & B200_FRAME_CCP) || !h->ccp.count || (h->ccp.off & 15) || end > nbytes || c.chroma_format_idc != 3)
             return fail(ctx, B200_EINVAL, "CCP section out of bounds (or not a 4:4:4 picture)");
     }
-    if (h->ictb.count) {                                         // CTB index of the intra list (contents are checked by the kernel that uses them)
-        if ((h->ictb.off & 15) || (uint64_t)h->ictb.off + 4ull * h->ictb.count > nbytes || h->ictb.count != (uint32_t)(ctx->ctb_w * ctx->ctb_h + 1))
-            return fail(ctx, B200_EINVAL, "intra CTB index out of bounds / of the wrong size");
-    }
+    if (h->reserved_section.off || h->reserved_section.count) return fail(ctx, B200_EINVAL, "reserved header section is not zero");
     if (h->dbd.count) {                                          // deblocking parameters derived on the device: header + arrays inside the section
         const uint64_t sec_bytes = 4ull * h->dbd.count, end = (uint64_t)h->dbd.off + sec_bytes;
         if ((h->dbd.off & 15) || end > nbytes || sec_bytes < sizeof(B200DbdHeader)) return fail(ctx, B200_EINVAL, "DBD section out of bounds");
@@ -712,17 +706,7 @@ extern "C" int b200_frame_execute_ex(B200Ctx *ctx, int arena, int cur_slot, cons
         ctx->launches += launch_ccp(st, (const B200CcpRec *)(a.dev + h.ccp.off), (int)h.ccp.count, L.parked, cur, bd, L.counter, ctx->arena_bytes);
     if (pf) CU(cudaEventRecord(ctx->prof[2], st));
     if (tr) CU(cudaEventRecord(tr->ev[2], st));
-    // K3 intra: CTB-granular when the list comes with its CTB index (constrained_intra_pred pictures keep the TU-granular stage)
-    if (h.ictb.count && h.sec[B200_SEC_INTRA].count && !((h.flags & B200_FRAME_CIP) && h.cip.count)) {
-        if (!L.ictb_done) {
-            CU(cudaMalloc(&L.ictb_done, sizeof(uint32_t) * (size_t)ctx->ctb_w * ctx->ctb_h));
-            CU(cudaMemsetAsync(L.ictb_done, 0, sizeof(uint32_t) * (size_t)ctx->ctb_w * ctx->ctb_h, st));
-        }
-        if (++L.ictb_gen == 0) { CU(cudaMemsetAsync(L.ictb_done, 0, sizeof(uint32_t) * (size_t)ctx->ctb_w * ctx->ctb_h, st)); L.ictb_gen = 1; }
-        ctx->launches += launch_intra_ctb(st, (const B200IntraRec *)(a.dev + h.sec[B200_SEC_INTRA].off), (int)h.sec[B200_SEC_INTRA].count, (const uint32_t *)(a.dev + h.ictb.off),
-                                          ctx->ctb_w, ctx->ctb_h, ctx->cfg.log2_ctb_size, ctx->cfg.chroma_format_idc, L.parked, ctx->arena_bytes / 2, cur, bd, L.counter,
-                                          L.ictb_done, L.ictb_gen);
-    } else
+    // K3 intra
     ctx->launches += launch_intra(st, (const B200IntraRec *)(a.dev + h.sec[B200_SEC_INTRA].off), (int)h.sec[B200_SEC_INTRA].count, L.parked, cur, bd,
                                   L.flags, ctx->flag_stride, L.counter,
                                   (h.flags & B200_FRAME_CIP) && h.cip.count ? (const uint32_t *)(a.dev + h.cip.off) : nullptr, &a.cip_hdr, ctx->cfg.chroma_format_idc);

@@ -395,7 +395,11 @@ __global__ void __launch_bounds__(128) k_ccp(const B200CcpRec *__restrict__ recs
 // Reference window staged in shared memory with clamped addressing (== emulated_edge_mc),
 // separable FIR with the 14-bit intermediate of the reference.
 // --------------------------------------------------------------------------------------------
-#include "k_mc.cuh"
+#define MC_WIN_MAX 640      // (32+7+1) x 15 = 600, (16+7+1) x 23 = 552, + slack for padded reads
+#define MC_TMP_MAX 512      // 15 x 32, 23 x 16
+template <int GS> struct McSmem;
+template <> struct McSmem<32> { static constexpr int WIN = MC_WIN_MAX, TMP = MC_TMP_MAX; };
+template <> struct McSmem<8>  { static constexpr int WIN = 256 /* 15 x 16 */, TMP = 160 /* 15 x 8 */; };
 
 // K1a: prediction blocks -> tiles.  The host records ONE record per table call (a block of up to 64x64 samples, hevc.c:1641-1949)
 // instead of cutting it into up to 24 tiles itself (6-9 % of the hooked decoder's host time, and 60 % of the upload of a lightly
@@ -463,18 +467,20 @@ __device__ __forceinline__ int ref_slot_of(const RefTable &rt, int i)
     return (int)((w >> (8 * (i & 7))) & 0xff);
 }
 
-
+// a reference plane, from the DPB's descriptor table
+__device__ __forceinline__ PlaneDesc ref_plane(const FrameDesc *__restrict__ dpb, int slot, int plane)
+{
+    return dpb[slot].p[plane];
+}
 // The DPB is one regular allocation (engine.cu: slot s starts at dpb + s * slot_bytes, same plane offsets in every slot), so a
-// reference plane can be described from kernel parameters instead of being loaded from the descriptor table in global
-// memory -- one dependent memory latency less per list and tile.  `slot_bytes` == 0 selects the table (B200_MC_DESC=0).
+// reference plane can also be described from kernel parameters instead of being loaded from the descriptor table in global
+// memory -- one dependent memory latency less per list and tile (k_mc_v4).
 struct DpbLayout {
     FrameDesc slot0;
     unsigned long long slot_bytes;
-    int tmp_pad;                // B200_MC_PAD (McGeom.ts)
 };
-__device__ __forceinline__ PlaneDesc ref_plane(const DpbLayout &L, const FrameDesc *__restrict__ dpb, int slot, int plane)
+__device__ __forceinline__ PlaneDesc ref_plane(const DpbLayout &L, int slot, int plane)
 {
-    if (!L.slot_bytes) return dpb[slot].p[plane];
     PlaneDesc d = plane_of(L.slot0, plane);
     d.base += (size_t)slot * L.slot_bytes;
     return d;
@@ -484,8 +490,7 @@ struct McGeom {
     int w, h;
     int wsh, parts, rows_per;   // stage B: lane = column (1 << wsh per row group), `parts` row groups of rows_per rows
     int wpad, lsh, q;           // stage A: 4 outputs per lane, q quads per row, (1 << lsh) lanes per row
-    int ts;                     // row stride of the 16-bit intermediate in shared memory: wpad, or wpad + 2 (B200_MC_PAD=1: the row
-                                // groups of stage B then start on different banks; with a stride of 16 or 8 samples they collide)
+    int ts;                     // row stride of the 16-bit intermediate in shared memory (= wpad)
 };
 
 // A tile is processed by a GROUP of GS lanes: GS = 32 (one warp per tile) for the big tiles, GS = 8 (four tiles per
@@ -496,17 +501,17 @@ struct McGeom {
 // One reference list of one tile: fills val[j] (j < rows_per) with the 14-bit intermediate of sample
 // (x = gl & (wpw-1), y = part * rows_per + j), exactly the value put_hevc_{q,e}pel* would hold.
 // the window of reference samples one list of one tile needs, as it lies in shared memory
-struct McWin1 {
+struct McWin {
     int R;                      // rows
     int ox, oy;                 // picture position of its first sample (before the even alignment)
     int skew, ax;               // origin aligned down to an even sample: ax = ox - skew
     int np, Ws;                 // sample pairs per row, shared-memory row stride (samples)
 };
 template <int TAPS>
-__device__ __forceinline__ McWin1 mc_win1(int sx, int sy, int mx, int my, const McGeom &g)
+__device__ __forceinline__ McWin mc_win(int sx, int sy, int mx, int my, const McGeom &g)
 {
     constexpr int BEFORE = TAPS == 8 ? 3 : 1;
-    McWin1 m;
+    McWin m;
     const int C = g.w + (mx ? TAPS - 1 : 0);
     m.R = g.h + (my ? TAPS - 1 : 0);
     m.ox = sx - (mx ? BEFORE : 0); m.oy = sy - (my ? BEFORE : 0);
@@ -514,13 +519,13 @@ __device__ __forceinline__ McWin1 mc_win1(int sx, int sy, int mx, int my, const 
     m.np = (C + m.skew + 1) >> 1; m.Ws = 2 * m.np;
     return m;
 }
-__device__ __forceinline__ bool mc_win1_interior(const McWin1 &m, const PlaneDesc &rp)
+__device__ __forceinline__ bool mc_win_interior(const McWin &m, const PlaneDesc &rp)
 {
     return m.ax >= 0 && m.ax + m.Ws <= rp.w && m.oy >= 0 && m.oy + m.R <= rp.h;
 }
 // window hangs over the picture border: clamp sample by sample (== emulated_edge_mc)
 template <typename PIX, int GS>
-__device__ __forceinline__ void mc_win1_clamped(const McWin1 &m, const PlaneDesc &rp, int gl, uint16_t *win)
+__device__ __forceinline__ void mc_win_clamped(const McWin &m, const PlaneDesc &rp, int gl, uint16_t *win)
 {
     for (int i = gl; i < m.R * m.Ws; i += GS) {
         const int r = i / m.Ws, cc = i - r * m.Ws;
@@ -537,17 +542,17 @@ __device__ __forceinline__ uint32_t mc_ld_pair(const uint8_t *src)          // t
 }
 
 template <int TAPS, int GS, typename WT>
-__device__ __forceinline__ void mc_list_fir(const McWin1 &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
+__device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
                                             const WT *win, int16_t *tmp, int (&val)[8]);
 
 template <typename PIX, int TAPS, int GS>
 __device__ __forceinline__ void mc_list(const PlaneDesc &rp, int sx, int sy, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
                                         uint16_t *win, int16_t *tmp, int (&val)[8])
 {
-    const McWin1 m = mc_win1<TAPS>(sx, sy, mx, my, g);
+    const McWin m = mc_win<TAPS>(sx, sy, mx, my, g);
     const int R = m.R, np = m.np, ax = m.ax, oy = m.oy;
     __syncwarp(gmask);
-    if (mc_win1_interior(m, rp)) {
+    if (mc_win_interior(m, rp)) {
         // interior: one 2-sample load per lane, 1 or 2 rows per pass, no clamping
         const int lpr = np <= GS / 2 ? GS / 2 : GS;         // lanes per window row
         const int pi = gl & (lpr - 1), rsub = gl >= lpr ? 1 : 0, rstep = GS / lpr;
@@ -559,7 +564,7 @@ __device__ __forceinline__ void mc_list(const PlaneDesc &rp, int sx, int sy, int
                 src += (size_t)rstep * rp.pitch; dst += rstep * np;
             }
         }
-    } else mc_win1_clamped<PIX, GS>(m, rp, gl, win);
+    } else mc_win_clamped<PIX, GS>(m, rp, gl, win);
     __syncwarp(gmask);
     mc_list_fir<TAPS, GS>(m, mx, my, g, bd, gl, gmask, win, tmp, val);
 }
@@ -567,7 +572,7 @@ __device__ __forceinline__ void mc_list(const PlaneDesc &rp, int sx, int sy, int
 // the FIRs of one list on a window that is complete in shared memory (WT: uint16_t, or the picture's own sample type for the
 // windows k_mc_v4 copies asynchronously)
 template <int TAPS, int GS, typename WT>
-__device__ __forceinline__ void mc_list_fir(const McWin1 &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
+__device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
                                             const WT *win, int16_t *tmp, int (&val)[8])
 {
     const int R = m.R, Ws = m.Ws, skew = m.skew;
@@ -634,15 +639,15 @@ __device__ __forceinline__ void mc_list_fir(const McWin1 &m, int mx, int my, con
     }
 }
 
-// ---- K1, default version: scalar FIRs (one IMAD per tap) ----
+// ---- K1, default version (k_mc): scalar FIRs (one IMAD per tap) ----
 // B200McRec fields straight from the two 16-byte halves of the record
-struct McRec1 {
+struct McRec {
     int dx, dy, w, h, plane, flags, sx0, sy0, sx1, sy1, ref0, ref1, frac0, frac1, w0, w1, o0, o1, denom;
 };
 template <int GS>
-__device__ __forceinline__ McRec1 mc_rec1(const int4 ra, const int4 rb)
+__device__ __forceinline__ McRec mc_rec(const int4 ra, const int4 rb)
 {
-    McRec1 t;
+    McRec t;
     const int mxy = ra.x, whpf = ra.y;
     t.dx = mxy & 0xffff; t.dy = (unsigned)mxy >> 16;
     t.w = whpf & 0xff; t.h = (whpf >> 8) & 0xff;
@@ -655,7 +660,7 @@ __device__ __forceinline__ McRec1 mc_rec1(const int4 ra, const int4 rb)
     return t;
 }
 template <int GS>
-__device__ __forceinline__ McGeom mc_geom1(int w, int h, int pad = 0)
+__device__ __forceinline__ McGeom mc_geom(int w, int h)
 {
     McGeom g;
     g.w = w; g.h = h;
@@ -665,12 +670,12 @@ __device__ __forceinline__ McGeom mc_geom1(int w, int h, int pad = 0)
     g.wpad = (w + 3) & ~3;
     g.q = g.wpad >> 2;
     g.lsh = g.q <= 1 ? 0 : g.q <= 2 ? 1 : g.q <= 4 ? 2 : 3;
-    g.ts = g.wpad + (pad && g.wpad < 32 ? 2 : 0);
+    g.ts = g.wpad;
     return g;
 }
 // combine the lists' 14-bit intermediates (hevcdsp_template.c put_hevc_*_uni / _bi / _w) and store the tile
 template <typename PIX>
-__device__ __forceinline__ void mc_store1(const McRec1 &t, const McGeom &g, const PlaneDesc &dp, int bd, int gl, const int (&v0)[8], const int (&v1)[8])
+__device__ __forceinline__ void mc_store(const McRec &t, const McGeom &g, const PlaneDesc &dp, int bd, int gl, const int (&v0)[8], const int (&v1)[8])
 {
     const bool bi = t.flags & B200_MCF_BI, weighted = t.flags & B200_MCF_WEIGHTED;
     const int w = t.w, h = t.h, w0 = t.w0, w1 = t.w1, o0 = t.o0, o1 = t.o1, denom = t.denom;
@@ -703,8 +708,8 @@ __device__ __forceinline__ void mc_store1(const McRec1 &t, const McGeom &g, cons
 }
 
 template <typename PIX, int GS>
-__global__ void __launch_bounds__(256) k_mc_v1(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                            const uint32_t *__restrict__ gate, DpbLayout lay)
+__global__ void __launch_bounds__(256) k_mc(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
+                                         const uint32_t *__restrict__ gate)
 {
     if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
     constexpr int NG = 256 / GS;                           // groups per CTA
@@ -715,21 +720,21 @@ __global__ void __launch_bounds__(256) k_mc_v1(const B200McRec *__restrict__ rec
     const int ri = blockIdx.x * NG + grp;
     if (ri >= count) return;                               // whole groups leave: the barriers are group-local
     const int4 *rp4 = reinterpret_cast<const int4 *>(recs + ri);
-    const McRec1 t = mc_rec1<GS>(__ldg(rp4), __ldg(rp4 + 1));
+    const McRec t = mc_rec<GS>(__ldg(rp4), __ldg(rp4 + 1));
     const bool chroma = t.flags & B200_MCF_CHROMA, bi = t.flags & B200_MCF_BI;
-    const McGeom g = mc_geom1<GS>(t.w, t.h, lay.tmp_pad);
+    const McGeom g = mc_geom<GS>(t.w, t.h);
     int v0[8], v1[8];
     {
-        const PlaneDesc rp = ref_plane(lay, dpb, ref_slot_of(rt, t.ref0), t.plane);
+        const PlaneDesc rp = ref_plane(dpb, ref_slot_of(rt, t.ref0), t.plane);
         if (chroma) mc_list<PIX, 4, GS>(rp, t.sx0, t.sy0, t.frac0 & 15, t.frac0 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v0);
         else        mc_list<PIX, 8, GS>(rp, t.sx0, t.sy0, t.frac0 & 15, t.frac0 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v0);
     }
     if (bi) {
-        const PlaneDesc rp = ref_plane(lay, dpb, ref_slot_of(rt, t.ref1), t.plane);
+        const PlaneDesc rp = ref_plane(dpb, ref_slot_of(rt, t.ref1), t.plane);
         if (chroma) mc_list<PIX, 4, GS>(rp, t.sx1, t.sy1, t.frac1 & 15, t.frac1 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v1);
         else        mc_list<PIX, 8, GS>(rp, t.sx1, t.sy1, t.frac1 & 15, t.frac1 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v1);
     }
-    mc_store1<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
+    mc_store<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
 }
 
 // ---- K1, version 3 (B200_MC=3): the arithmetic of the default version, but the window loads of BOTH lists are issued before
@@ -739,7 +744,7 @@ __global__ void __launch_bounds__(256) k_mc_v1(const B200McRec *__restrict__ rec
 // Here a lane issues up to 2 x 15 loads back to back into registers, then commits them to the two shared-memory windows.
 #define MC3_PASSES 15          // 32x8 tiles: 15 rows, one per pass; 16x16 tiles: 23 rows, two per pass; 8-lane groups: <= 15 rows
 template <typename PIX, int GS>
-__device__ __forceinline__ void mc3_issue(const McWin1 &m, const PlaneDesc &rp, int gl, uint32_t (&v)[MC3_PASSES])
+__device__ __forceinline__ void mc3_issue(const McWin &m, const PlaneDesc &rp, int gl, uint32_t (&v)[MC3_PASSES])
 {
     const int np = m.np;
     const int lpr = np <= GS / 2 ? GS / 2 : GS;         // lanes per window row
@@ -751,7 +756,7 @@ __device__ __forceinline__ void mc3_issue(const McWin1 &m, const PlaneDesc &rp, 
     for (int i = 0; i < MC3_PASSES; i++) v[i] = mc_ld_pair<PIX>(src + (size_t)min(rsub + i * rstep, m.R - 1) * rp.pitch);
 }
 template <typename PIX, int GS>
-__device__ __forceinline__ void mc3_commit(const McWin1 &m, const PlaneDesc &rp, int gl, const uint32_t (&v)[MC3_PASSES], uint16_t *win)
+__device__ __forceinline__ void mc3_commit(const McWin &m, const PlaneDesc &rp, int gl, const uint32_t (&v)[MC3_PASSES], uint16_t *win)
 {
     const int np = m.np;
     const int lpr = np <= GS / 2 ? GS / 2 : GS;
@@ -768,7 +773,7 @@ __device__ __forceinline__ void mc3_commit(const McWin1 &m, const PlaneDesc &rp,
 
 template <typename PIX, int GS>
 __global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                            const uint32_t *__restrict__ gate, DpbLayout lay)
+                                            const uint32_t *__restrict__ gate)
 {
     if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
     constexpr int NG = 256 / GS;                           // groups per CTA
@@ -779,21 +784,21 @@ __global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ 
     const int ri = blockIdx.x * NG + grp;
     if (ri >= count) return;                               // whole groups leave: the barriers are group-local
     const int4 *rp4 = reinterpret_cast<const int4 *>(recs + ri);
-    const McRec1 t = mc_rec1<GS>(__ldg(rp4), __ldg(rp4 + 1));
+    const McRec t = mc_rec<GS>(__ldg(rp4), __ldg(rp4 + 1));
     const bool chroma = t.flags & B200_MCF_CHROMA, bi = t.flags & B200_MCF_BI;
-    const McGeom g = mc_geom1<GS>(t.w, t.h);
+    const McGeom g = mc_geom<GS>(t.w, t.h);
     const int mx0 = t.frac0 & 15, my0 = t.frac0 >> 4, mx1 = t.frac1 & 15, my1 = t.frac1 >> 4;
-    const PlaneDesc rp0 = ref_plane(lay, dpb, ref_slot_of(rt, t.ref0), t.plane);
-    const PlaneDesc rp1 = bi ? ref_plane(lay, dpb, ref_slot_of(rt, t.ref1), t.plane) : rp0;
-    const McWin1 m0 = chroma ? mc_win1<4>(t.sx0, t.sy0, mx0, my0, g) : mc_win1<8>(t.sx0, t.sy0, mx0, my0, g);
-    const McWin1 m1 = chroma ? mc_win1<4>(t.sx1, t.sy1, mx1, my1, g) : mc_win1<8>(t.sx1, t.sy1, mx1, my1, g);
-    const bool in0 = mc_win1_interior(m0, rp0), in1 = bi && mc_win1_interior(m1, rp1);      // uniform over the group
+    const PlaneDesc rp0 = ref_plane(dpb, ref_slot_of(rt, t.ref0), t.plane);
+    const PlaneDesc rp1 = bi ? ref_plane(dpb, ref_slot_of(rt, t.ref1), t.plane) : rp0;
+    const McWin m0 = chroma ? mc_win<4>(t.sx0, t.sy0, mx0, my0, g) : mc_win<8>(t.sx0, t.sy0, mx0, my0, g);
+    const McWin m1 = chroma ? mc_win<4>(t.sx1, t.sy1, mx1, my1, g) : mc_win<8>(t.sx1, t.sy1, mx1, my1, g);
+    const bool in0 = mc_win_interior(m0, rp0), in1 = bi && mc_win_interior(m1, rp1);      // uniform over the group
     uint16_t *win0 = win_s[grp][0], *win1 = win_s[grp][1];
     uint32_t r0[MC3_PASSES], r1[MC3_PASSES];
     if (in0) mc3_issue<PIX, GS>(m0, rp0, gl, r0);
     if (in1) mc3_issue<PIX, GS>(m1, rp1, gl, r1);
-    if (!in0) mc_win1_clamped<PIX, GS>(m0, rp0, gl, win0);
-    if (bi && !in1) mc_win1_clamped<PIX, GS>(m1, rp1, gl, win1);
+    if (!in0) mc_win_clamped<PIX, GS>(m0, rp0, gl, win0);
+    if (bi && !in1) mc_win_clamped<PIX, GS>(m1, rp1, gl, win1);
     if (in0) mc3_commit<PIX, GS>(m0, rp0, gl, r0, win0);
     if (in1) mc3_commit<PIX, GS>(m1, rp1, gl, r1, win1);
     __syncwarp(gmask);
@@ -805,11 +810,11 @@ __global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ 
         if (chroma) mc_list_fir<4, GS>(m1, mx1, my1, g, bd, gl, gmask, win1, tmp_s[grp], v1);
         else        mc_list_fir<8, GS>(m1, mx1, my1, g, bd, gl, gmask, win1, tmp_s[grp], v1);
     }
-    mc_store1<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
+    mc_store<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
 }
 
 
-// ---- K1, version 4 (B200_MC=4): the arithmetic of the default version behind a software pipeline.  ncu on versions 1-3: the
+// ---- K1, version 4 (B200_MC=4): the arithmetic of the default version behind a software pipeline.  ncu on versions 1 and 3: the
 // stage waits for its window loads (long scoreboard 9 per issue, DRAM at 10 %); a tile pays record -> descriptor -> window as
 // dependent round trips, in 4-byte loads, and nothing overlaps them.  Here the groups are PERSISTENT: while a group filters
 // tile k from one shared-memory buffer, the windows of both lists of tile k + 1 arrive in the other one through 16-byte
@@ -834,12 +839,12 @@ template <int GS> struct Mc4Smem;
 template <> struct Mc4Smem<32> { static constexpr int WIN_BYTES = 1536, TMP = MC_TMP_MAX, THREADS = 256; };   // (16+7) rows x 4 chunks, 15 rows x 6 chunks
 template <> struct Mc4Smem<8>  { static constexpr int WIN_BYTES = 768,  TMP = 128,        THREADS = 128; };   // 15 rows x 3 chunks
 
-// window of one list of one tile in the chunked layout (fields named like McWin1: the FIR code is shared)
+// window of one list of one tile in the chunked layout (fields named like McWin: the FIR code is shared)
 template <typename PIX, int TAPS>
-__device__ __forceinline__ McWin1 mc4_win(int sx, int sy, int mx, int my, const McGeom &g, const PlaneDesc &rp, bool &interior)
+__device__ __forceinline__ McWin mc4_win(int sx, int sy, int mx, int my, const McGeom &g, const PlaneDesc &rp, bool &interior)
 {
     constexpr int BEFORE = TAPS == 8 ? 3 : 1, SPC = 16 / (int)sizeof(PIX);
-    McWin1 m;
+    McWin m;
     const int C = g.w + (mx ? TAPS - 1 : 0);
     m.R = g.h + (my ? TAPS - 1 : 0);
     m.ox = sx - (mx ? BEFORE : 0); m.oy = sy - (my ? BEFORE : 0);
@@ -855,7 +860,7 @@ __device__ __forceinline__ McWin1 mc4_win(int sx, int sy, int mx, int my, const 
     return m;
 }
 template <typename PIX, int GS>
-__device__ __forceinline__ void mc4_fill(const McWin1 &m, bool interior, const PlaneDesc &rp, int gl, PIX *win)
+__device__ __forceinline__ void mc4_fill(const McWin &m, bool interior, const PlaneDesc &rp, int gl, PIX *win)
 {
     constexpr int SPC = 16 / (int)sizeof(PIX);
     if (interior) {
@@ -875,8 +880,8 @@ __device__ __forceinline__ void mc4_fill(const McWin1 &m, bool interior, const P
 }
 
 template <typename PIX, int GS>
-__global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                                               const uint32_t *__restrict__ gate, DpbLayout lay)
+__global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec *__restrict__ recs, int count, FrameDesc cur, RefTable rt, int bd, const uint32_t *__restrict__ gate,
+                                                               DpbLayout lay)
 {
     if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
     constexpr int THREADS = Mc4Smem<GS>::THREADS, NG = THREADS / GS, WB = Mc4Smem<GS>::WIN_BYTES;
@@ -893,21 +898,21 @@ __global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec 
     int ti = blockIdx.x * NG + grp;
     if (ti >= count) return;                                                        // whole groups leave: the barriers are group-local
 
-    struct Tile { McRec1 t; McGeom g; McWin1 m0, m1; bool bi, chroma; };
+    struct Tile { McRec t; McGeom g; McWin m0, m1; bool bi, chroma; };
     auto decode = [&](const int4 ra, const int4 rb) {
         Tile T;
-        T.t = mc_rec1<GS>(ra, rb);
+        T.t = mc_rec<GS>(ra, rb);
         T.chroma = T.t.flags & B200_MCF_CHROMA; T.bi = T.t.flags & B200_MCF_BI;
-        T.g = mc_geom1<GS>(T.t.w, T.t.h);
+        T.g = mc_geom<GS>(T.t.w, T.t.h);
         return T;
     };
     auto issue = [&](Tile &T, int buf) {                                            // windows of both lists -> buffer `buf`
-        const PlaneDesc rp0 = ref_plane(lay, dpb, ref_slot_of(rt, T.t.ref0), T.t.plane);
+        const PlaneDesc rp0 = ref_plane(lay, ref_slot_of(rt, T.t.ref0), T.t.plane);
         bool in0, in1 = false;
         T.m0 = T.chroma ? mc4_win<PIX, 4>(T.t.sx0, T.t.sy0, T.t.frac0 & 15, T.t.frac0 >> 4, T.g, rp0, in0) : mc4_win<PIX, 8>(T.t.sx0, T.t.sy0, T.t.frac0 & 15, T.t.frac0 >> 4, T.g, rp0, in0);
         mc4_fill<PIX, GS>(T.m0, in0, rp0, gl, reinterpret_cast<PIX *>(wbase + (size_t)(2 * buf) * WB));
         if (T.bi) {
-            const PlaneDesc rp1 = ref_plane(lay, dpb, ref_slot_of(rt, T.t.ref1), T.t.plane);
+            const PlaneDesc rp1 = ref_plane(lay, ref_slot_of(rt, T.t.ref1), T.t.plane);
             T.m1 = T.chroma ? mc4_win<PIX, 4>(T.t.sx1, T.t.sy1, T.t.frac1 & 15, T.t.frac1 >> 4, T.g, rp1, in1) : mc4_win<PIX, 8>(T.t.sx1, T.t.sy1, T.t.frac1 & 15, T.t.frac1 >> 4, T.g, rp1, in1);
             mc4_fill<PIX, GS>(T.m1, in1, rp1, gl, reinterpret_cast<PIX *>(wbase + (size_t)(2 * buf + 1) * WB));
         }
@@ -928,7 +933,7 @@ __global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec 
         cp_async_wait<1>();                                                         // this tile's windows have landed (the next tile's may not)
         __syncwarp(gmask);
         const PIX *w0 = reinterpret_cast<const PIX *>(wbase + (size_t)(2 * (it & 1)) * WB), *w1 = reinterpret_cast<const PIX *>(wbase + (size_t)(2 * (it & 1) + 1) * WB);
-        const McRec1 &t = cur_t.t;
+        const McRec &t = cur_t.t;
         int v0[8], v1[8];
         if (cur_t.chroma) mc_list_fir<4, GS>(cur_t.m0, t.frac0 & 15, t.frac0 >> 4, cur_t.g, bd, gl, gmask, w0, tmp, v0);
         else              mc_list_fir<8, GS>(cur_t.m0, t.frac0 & 15, t.frac0 >> 4, cur_t.g, bd, gl, gmask, w0, tmp, v0);
@@ -937,49 +942,12 @@ __global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec 
             if (cur_t.chroma) mc_list_fir<4, GS>(cur_t.m1, t.frac1 & 15, t.frac1 >> 4, cur_t.g, bd, gl, gmask, w1, tmp, v1);
             else              mc_list_fir<8, GS>(cur_t.m1, t.frac1 & 15, t.frac1 >> 4, cur_t.g, bd, gl, gmask, w1, tmp, v1);
         }
-        mc_store1<PIX>(t, cur_t.g, plane_of(cur, t.plane), bd, gl, v0, v1);
+        mc_store<PIX>(t, cur_t.g, plane_of(cur, t.plane), bd, gl, v0, v1);
         __syncwarp(gmask);                                                          // everybody is done with this buffer and tmp
         cur_t = next_t;
     }
 }
 
-
-// K1, experimental version (B200_MC=2): the phases of k_mc.cuh (IDP.2A FIRs on packed sample pairs) with group-local barriers between them
-template <typename PIX, int GS>
-__global__ void __launch_bounds__(256, 4) k_mc(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                            const uint32_t *__restrict__ gate, DpbLayout lay)
-{
-    if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
-    constexpr int NG = 256 / GS;                           // groups per CTA
-    __shared__ __align__(16) uint16_t win_s[NG][McSmem<GS>::WIN];
-    __shared__ __align__(16) int16_t tmp_s[NG][McSmem<GS>::TMP];
-    const int grp = threadIdx.x / GS, gl = threadIdx.x & (GS - 1);
-    const unsigned gmask = GS == 32 ? 0xffffffffu : (((1u << GS) - 1u) << ((threadIdx.x & 31) & ~(GS - 1)));
-    const int ri = blockIdx.x * NG + grp;
-    if (ri >= count) return;                               // whole groups leave: the barriers are group-local
-    const int4 *rp4 = reinterpret_cast<const int4 *>(recs + ri);
-    const McTile t = mc_decode<GS>(__ldg(rp4), __ldg(rp4 + 1));
-    const bool chroma = t.flags & B200_MCF_CHROMA, bi = t.flags & B200_MCF_BI;
-    uint16_t *win = win_s[grp];
-    int16_t *tmp = tmp_s[grp];
-    int v0[8], v1[8];
-#pragma unroll
-    for (int list = 0; list < 2; list++) {
-        if (list && !bi) break;
-        const PlaneDesc rp = ref_plane(lay, dpb, ref_slot_of(rt, list ? t.ref1 : t.ref0), t.plane);
-        const int sx = list ? t.sx1 : t.sx0, sy = list ? t.sy1 : t.sy0, fr = list ? t.frac1 : t.frac0, mx = fr & 15, my = fr >> 4;
-        int (&v)[8] = list ? v1 : v0;
-        __syncwarp(gmask);                                 // the previous list's readers are done with win / tmp
-        if (chroma) mc_load_window<PIX, 4, GS>(rp, t, sx, sy, mx, my, gl, win); else mc_load_window<PIX, 8, GS>(rp, t, sx, sy, mx, my, gl, win);
-        __syncwarp(gmask);
-        if (mx) {
-            if (chroma) mc_stage_a<4, GS>(t, sx, sy, mx, my, bd, gl, win, tmp); else mc_stage_a<8, GS>(t, sx, sy, mx, my, bd, gl, win, tmp);
-            __syncwarp(gmask);
-        }
-        if (chroma) mc_stage_b<4, GS>(t, sx, sy, mx, my, bd, gl, win, tmp, v); else mc_stage_b<8, GS>(t, sx, sy, mx, my, bd, gl, win, tmp, v);
-    }
-    mc_store<PIX>(t, plane_of(cur, t.plane), bd, gl, v0, v1);
-}
 
 // --------------------------------------------------------------------------------------------
 // K3: intra prediction.  Persistent warps take TUs in dependency-level order from an atomic counter.
@@ -1065,32 +1033,6 @@ __global__ void k_intra_edges_init(FrameDesc f, IntraEdges ed)
     const uint2 bot = edge_pack(b[0], b[1], b[2], b[3]), rgt = edge_pack(r0, r1, r2, b[3]);
     uint4 *dst = reinterpret_cast<uint4 *>(edges_of(ed, plane) + 2 * ((size_t)uy * estride_of(ed, plane) + ux));
     *dst = make_uint4(bot.x, bot.y, rgt.x, rgt.y);
-}
-
-// The same, driven by the intra records: only the units an intra TU can read (the row above from the up-left corner to the
-// end of the up-right block, the column to the left down to the end of the bottom-left block) are initialised -- a B
-// picture with 8 % intra blocks touches a few per cent of the picture instead of reading all of it (25 MB at 4K).
-// One warp per record, lane k = unit k of the 4u + 1 neighbours.  Units that belong to another intra TU get a record from
-// the picture as well; k_intra_prepass, which runs after this kernel, marks them "not valid yet" again.
-template <typename PIX>
-__global__ void k_intra_edges_init_sparse(const B200IntraRec *__restrict__ recs, int count, FrameDesc f, IntraEdges ed, const uint32_t *__restrict__ gate)
-{
-    if (__ldg(gate + 1)) return;
-    const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (i >= count) return;
-    const B200IntraRec r = decode_intra(__ldg(reinterpret_cast<const int4 *>(recs + i)));
-    const PlaneDesc pd = plane_of(f, r.plane);
-    const int u = 1 << (r.log2 - 2), ux0 = r.x >> 2, uy0 = r.y >> 2;
-    for (int k = lane; k < 4 * u + 1; k += 32) {
-        // k = 0 .. 2u: row above, from the corner; k = 2u + 1 .. 4u: column to the left, top down
-        const int ux = k <= 2 * u ? ux0 - 1 + k : ux0 - 1, uy = k <= 2 * u ? uy0 - 1 : uy0 + (k - 2 * u - 1);
-        if (ux < 0 || uy < 0 || 4 * ux >= pd.w || 4 * uy >= pd.h) continue;
-        const PIX *b = px_ptr<PIX>(pd, 4 * ux, 4 * uy + 3);
-        const int r0 = *px_ptr<PIX>(pd, 4 * ux + 3, 4 * uy), r1 = *px_ptr<PIX>(pd, 4 * ux + 3, 4 * uy + 1), r2 = *px_ptr<PIX>(pd, 4 * ux + 3, 4 * uy + 2);
-        const uint2 bot = edge_pack(b[0], b[1], b[2], b[3]), rgt = edge_pack(r0, r1, r2, b[3]);
-        uint4 *dst = reinterpret_cast<uint4 *>(edges_of(ed, r.plane) + 2 * ((size_t)uy * estride_of(ed, r.plane) + ux));
-        *dst = make_uint4(bot.x, bot.y, rgt.x, rgt.y);
-    }
 }
 
 // units an intra TU of this picture will write: not valid yet
@@ -1460,8 +1402,6 @@ __global__ void __launch_bounds__(128) k_intra(const B200IntraRec *__restrict__ 
     }
 }
 
-#include "k_intra_ctb.cuh"
-
 // --------------------------------------------------------------------------------------------
 // K4: deblocking, both directions in ONE pass (k_deblock.cuh: one thread per 4-line edge segment).
 // --------------------------------------------------------------------------------------------
@@ -1559,57 +1499,45 @@ int launch_mc(cudaStream_t st, const B200McRec *recs, int count, int n_big, cons
               const FrameDesc &slot0, unsigned long long slot_bytes)
 {
     if (!count) return 0;
-    // B200_MC_DESC=1: reference planes described from kernel parameters (see DpbLayout); default 0 = descriptor table
-    static const bool by_param = getenv("B200_MC_DESC") && atoi(getenv("B200_MC_DESC"));
-    static const int tmp_pad = getenv("B200_MC_PAD") ? atoi(getenv("B200_MC_PAD")) : 0;
-    DpbLayout lay;
-    lay.slot0 = slot0; lay.slot_bytes = by_param ? slot_bytes : 0ull; lay.tmp_pad = tmp_pad;
-    // 1 = scalar FIRs, one IMAD per tap (default); 2 = IDP.2A on packed pairs (k_mc.cuh), bit-exact; its pair shuffles and
-    // 16-bit interleaved stores add instructions the halved multiplies have to pay back.
-    // 3 = version 1's arithmetic with the window loads of both lists issued back to back (k_mc_v3).
-    // 4 = persistent groups, windows double-buffered through 16-byte cp.async, descriptors from kernel parameters (k_mc_v4)
+    // 1 = scalar FIRs, one IMAD per tap (default, k_mc); 3 = the same arithmetic with the window loads of both lists issued back
+    // to back (k_mc_v3); 4 = persistent groups, windows double-buffered through 16-byte cp.async, descriptors from kernel
+    // parameters (k_mc_v4)
     static const int version = getenv("B200_MC") ? atoi(getenv("B200_MC")) : 1;
     DpbLayout lay4;
-    lay4.slot0 = slot0; lay4.slot_bytes = slot_bytes; lay4.tmp_pad = 0;
+    lay4.slot0 = slot0; lay4.slot_bytes = slot_bytes;
     int n = 0;
     const int n_small = count - n_big;
     if (n_big) {                        // one warp per tile
         const int grid = (n_big + 7) / 8;
-        if (version == 1) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v1<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v1<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
-        } else if (version == 3) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
+        if (version == 3) {
+            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
+            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
         } else if (version == 4) {
             constexpr int NG = Mc4Smem<32>::THREADS / 32, SM = NG * (4 * Mc4Smem<32>::WIN_BYTES + Mc4Smem<32>::TMP * 2);
             mc4_opt_in();
             const int g4 = mc4_grid((n_big + NG - 1) / NG);
-            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay4);
-            else        B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay4);
+            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint16_t, 32>)(recs, n_big, cur, rt, bd, gate, lay4);
+            else        B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint8_t, 32>)(recs, n_big, cur, rt, bd, gate, lay4);
         } else {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate, lay);
+            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
+            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
         }
         n++;
     }
     if (n_small) {                      // tiles of <= 8x8 samples: four per warp
         const int grid = (n_small + 31) / 32;
-        if (version == 1) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v1<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v1<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
-        } else if (version == 3) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
+        if (version == 3) {
+            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
+            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
         } else if (version == 4) {
             constexpr int NG = Mc4Smem<8>::THREADS / 8, SM = NG * (4 * Mc4Smem<8>::WIN_BYTES + Mc4Smem<8>::TMP * 2);
             mc4_opt_in();
             const int g4 = mc4_grid((n_small + NG - 1) / NG);
-            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay4);
-            else        B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay4);
+            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint16_t, 8>)(recs + n_big, n_small, cur, rt, bd, gate, lay4);
+            else        B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint8_t, 8>)(recs + n_big, n_small, cur, rt, bd, gate, lay4);
         } else {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate, lay);
+            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
+            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
         }
         n++;
     }
@@ -1650,18 +1578,9 @@ int launch_intra(cudaStream_t st, const B200IntraRec *recs, int count, const int
     IntraEdges ed;
     for (int p = 0; p < 3; p++) { ed.e[p] = edges[p]; ed.stride[p] = edge_stride[p]; }
     // counter[0] (ticket) and counter[1] (gate) were cleared when the picture entered its lane (engine.cu)
-    // B200_EDGES_SPARSE=1: initialise only the edge records intra TUs can read (record-driven) when the picture is mostly inter;
-    // default 0 = every unit of the picture
-    static const bool sparse_ok = getenv("B200_EDGES_SPARSE") && atoi(getenv("B200_EDGES_SPARSE"));
-    const long units = (long)(cur.p[0].w / 4) * (cur.p[0].h / 4) + 2l * (cur.p[1].w / 4) * (cur.p[1].h / 4);
-    if (sparse_ok && (long)count * 16 < units) {
-        if (bd > 8) B200_LAUNCH((count + 3) / 4, 128, 0, st, k_intra_edges_init_sparse<uint16_t>)(recs, count, cur, ed, counter);
-        else        B200_LAUNCH((count + 3) / 4, 128, 0, st, k_intra_edges_init_sparse<uint8_t>)(recs, count, cur, ed, counter);
-    } else {
-        const dim3 gi((cur.p[0].w / 4 + 127) / 128, cur.p[0].h / 4, 3);
-        if (bd > 8) B200_LAUNCH(gi, 128, 0, st, k_intra_edges_init<uint16_t>)(cur, ed);
-        else        B200_LAUNCH(gi, 128, 0, st, k_intra_edges_init<uint8_t>)(cur, ed);
-    }
+    const dim3 gi((cur.p[0].w / 4 + 127) / 128, cur.p[0].h / 4, 3);
+    if (bd > 8) B200_LAUNCH(gi, 128, 0, st, k_intra_edges_init<uint16_t>)(cur, ed);
+    else        B200_LAUNCH(gi, 128, 0, st, k_intra_edges_init<uint8_t>)(cur, ed);
     B200_LAUNCH((count + 255) / 256, 256, 0, st, k_intra_prepass)(recs, count, ed, counter);
     int grid = (count + 3) / 4;
     // persistent warps.  The list is sorted by dependency level, so the TUs that can run together are adjacent and a
@@ -1680,41 +1599,6 @@ int launch_intra(cudaStream_t st, const B200IntraRec *recs, int count, const int
     if (bd > 8) B200_LAUNCH(grid, 128, 0, st, k_intra<uint16_t>)(recs, count, pool, cur, bd, ed, counter, cd);
     else        B200_LAUNCH(grid, 128, 0, st, k_intra<uint8_t>)(recs, count, pool, cur, bd, ed, counter, cd);
     return 3;
-}
-
-// K3, CTB-granular (k_intra_ctb.cuh): `ctb_start` = the blob's ictb section, `done` = one flag per CTB (compared with `gen`)
-int launch_intra_ctb(cudaStream_t st, const B200IntraRec *recs, int count, const uint32_t *ctb_start, int ctb_w, int ctb_h, int log2_ctb, int cfi, const int16_t *parked,
-                     unsigned long long parked_cap, const FrameDesc &cur, int bd, uint32_t *counter, uint32_t *done, uint32_t gen)
-{
-    if (!count) return 0;
-    IntraCtbArgs a;
-    a.recs = recs; a.ctb_start = ctb_start; a.parked = parked; a.counter = counter; a.done = done; a.gen = gen;
-    a.n_ctb = ctb_w * ctb_h; a.ctb_w = ctb_w; a.log2_ctb = log2_ctb; a.cfi = cfi; a.bd = bd; a.count = count; a.parked_cap = parked_cap;
-    const int ctb = 1 << log2_ctb;
-    int off = 0;
-    a.rec_off = off; off += ICTB_MAXREC * 16;
-    a.scratch_off = off; off += ICTB_WARPS * 400 * 4;
-    for (int p = 0; p < 3; p++) {
-        const int hs = p && cfi != 3, vs = p && cfi == 1, cw = ctb >> hs, ch = ctb >> vs;
-        const int ext = cw < 32 ? cw : 32;
-        a.tile_stride[p] = (1 + cw + ext + 1) & ~1;
-        a.tile_off[p] = off; off += ((a.tile_stride[p] * (ch + 1) * 2) + 15) & ~15;
-        a.rt_stride[p] = cw;
-        a.rt_off[p] = off; off += (cw * ch * 2 + 15) & ~15;
-    }
-    const int cap = 2 * sm_count();
-    int grid = a.n_ctb < cap ? a.n_ctb : cap;
-    static const int max_ctas = getenv("B200_INTRA_CTAS") ? atoi(getenv("B200_INTRA_CTAS")) : 0;
-    if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-    static bool attr_set[2] = { false, false };
-    if (!attr_set[bd > 8]) {                             // more than 48 KB of dynamic shared memory needs the opt-in, once per kernel
-        if (bd > 8) cudaFuncSetAttribute(k_intra_ctb<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        else        cudaFuncSetAttribute(k_intra_ctb<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-        attr_set[bd > 8] = true;
-    }
-    if (bd > 8) B200_LAUNCH(grid, ICTB_WARPS * 32, off, st, k_intra_ctb<uint16_t>)(a, cur);
-    else        B200_LAUNCH(grid, ICTB_WARPS * 32, off, st, k_intra_ctb<uint8_t>)(a, cur);
-    return 1;
 }
 
 int launch_deblock(cudaStream_t st, const uint16_t *grid, const B200DbkLayout &L, const FrameDesc &cur, int bd)

@@ -107,86 +107,6 @@ extern "C" int b200_intra_level_order(const B200IntraRec *recs, uint32_t n, int 
     return (int)maxl;
 }
 
-// Decode order -> CTB order for the CTB-granular intra stage (k_intra_ctb.cuh: one thread block per CTB, the CTB's samples in
-// shared memory).  Records are grouped by CTB (raster order: a CTB only ever reads CTBs in front of it) and, inside a CTB, sorted
-// by the dependency level counted INSIDE the CTB (neighbour units of other CTBs are complete before the block starts).
-// perm[new] = old; ctb_start[c] .. ctb_start[c + 1] = records of CTB c in the new order (nctb + 1 entries); level[new] = the
-// record's level (1 ..).  Input: decode order within every CTB.  Returns the largest level, or a negative error (> 255 levels:
-// B200_ENOTSUP, the caller falls back to the picture-wide level order).
-extern "C" int b200_intra_ctb_order(const B200IntraRec *recs, uint32_t n, int width, int height, int cfi, int log2_ctb,
-                                    uint32_t *perm, uint32_t *ctb_start, uint8_t *level_out)
-{
-    if (!recs || !perm || !ctb_start || !level_out || log2_ctb < 4 || log2_ctb > 6) return B200_EINVAL;
-    static thread_local std::vector<uint32_t> lvl[3], level, ctb_of, tmp, cnt;
-    const int ctb_w = (width + (1 << log2_ctb) - 1) >> log2_ctb, ctb_h = (height + (1 << log2_ctb) - 1) >> log2_ctb;
-    const uint32_t nctb = (uint32_t)ctb_w * ctb_h;
-    int fs[3], pw[3], ph[3];
-    // the unit maps stay allocated and CLEAN between calls: a picture with a few intra blocks must not pay for zeroing ~3 MB of maps,
-    // so whatever a call writes it resets before it returns (undo)
-    for (int p = 0; p < 3; p++) {
-        b200_plane_dims(width, height, cfi, p, &pw[p], &ph[p]);
-        fs[p] = pw[p] / 4 + 2;
-        const size_t need = (size_t)fs[p] * (ph[p] / 4 + 2);
-        if (lvl[p].size() != need) lvl[p].assign(need, 0);
-    }
-    auto undo = [&](uint32_t upto) {
-        for (uint32_t i = 0; i < upto; i++) {
-            const B200IntraRec &r = recs[i];
-            const int s = fs[r.plane], u = 1 << (r.log2 - 2), ux = r.x >> 2, uy = r.y >> 2;
-            for (int y = 0; y < u; y++) for (int x = 0; x < u; x++) lvl[r.plane][(size_t)(uy + y) * s + ux + x] = 0;
-        }
-    };
-    level.assign(n, 0); ctb_of.assign(n, 0);
-    uint32_t maxl = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        const B200IntraRec &r = recs[i];
-        if (r.plane > 2 || r.log2 < 2 || r.log2 > 5) { undo(i); return B200_EINVAL; }
-        const int p = r.plane, hs = p && cfi != 3, vs = p && cfi == 1;
-        const int lu = log2_ctb - 2;                                   // log2 of the CTB in luma units
-        std::vector<uint32_t> &L = lvl[p];
-        const int s = fs[p], u = 1 << (r.log2 - 2), ux = r.x >> 2, uy = r.y >> 2;
-        if ((size_t)(uy + u) * s + ux + u >= L.size() + s) { undo(i); return B200_EINVAL; }
-        const int cx = (ux << hs) >> lu, cy = (uy << vs) >> lu;
-        if (cx >= ctb_w || cy >= ctb_h) { undo(i); return B200_EINVAL; }
-        ctb_of[i] = (uint32_t)(cy * ctb_w + cx);
-        auto at = [&](int x, int y) -> uint32_t {                      // level of a unit, 0 when it lies in another CTB
-            if (x < 0 || y < 0) return 0;
-            if (((x << hs) >> lu) != cx || ((y << vs) >> lu) != cy) return 0;
-            const size_t idx = (size_t)y * s + x;
-            return idx < L.size() ? L[idx] : 0;
-        };
-        uint32_t m = 0;
-        if (r.flags & B200_INF_UP_LEFT) m = at(ux - 1, uy - 1);
-        {
-            int cnt_ = (r.flags & B200_INF_UP) ? u : 0, from = (r.flags & B200_INF_UP) ? 0 : u;
-            if (r.flags & B200_INF_UP_RIGHT) cnt_ = u + (r.top_right_size + 3) / 4;
-            for (int k = from; k < cnt_; k++) { const uint32_t v = at(ux + k, uy - 1); if (v > m) m = v; }
-        }
-        {
-            int cnt_ = (r.flags & B200_INF_LEFT) ? u : 0, from = (r.flags & B200_INF_LEFT) ? 0 : u;
-            if (r.flags & B200_INF_BOTTOM_LEFT) cnt_ = u + (r.bottom_left_size + 3) / 4;
-            for (int k = from; k < cnt_; k++) { const uint32_t v = at(ux - 1, uy + k); if (v > m) m = v; }
-        }
-        level[i] = m + 1;
-        if (level[i] > maxl) maxl = level[i];
-        for (int y = 0; y < u; y++) for (int x = 0; x < u; x++) L[(size_t)(uy + y) * s + ux + x] = m + 1;
-    }
-    undo(n);
-    if (maxl > 255) return B200_ENOTSUP;
-    // LSD radix: by level (stable), then by CTB (stable)
-    tmp.resize(n);
-    cnt.assign(maxl + 2, 0);
-    for (uint32_t i = 0; i < n; i++) cnt[level[i] + 1]++;
-    for (uint32_t k = 0; k <= maxl; k++) cnt[k + 1] += cnt[k];
-    for (uint32_t i = 0; i < n; i++) tmp[cnt[level[i]]++] = i;
-    for (uint32_t c = 0; c <= nctb; c++) ctb_start[c] = 0;
-    for (uint32_t i = 0; i < n; i++) ctb_start[ctb_of[i] + 1]++;
-    for (uint32_t c = 0; c < nctb; c++) ctb_start[c + 1] += ctb_start[c];
-    cnt.assign(ctb_start, ctb_start + nctb);
-    for (uint32_t k = 0; k < n; k++) { const uint32_t i = tmp[k]; const uint32_t at = cnt[ctb_of[i]]++; perm[at] = i; level_out[at] = (uint8_t)level[i]; }
-    return (int)maxl;
-}
-
 extern "C" int b200_rec_set_refs(B200Rec *r, const uint8_t *slots, int n)
 {
     if (!r || !r->open || n < 0 || n > 16 || (n && !slots)) return B200_EINVAL;
@@ -210,7 +130,7 @@ extern "C" uint64_t b200_worst_blob_bytes(const B200Config *c)
     const uint64_t nctb = (uint64_t)((c->width + ctb - 1) >> c->log2_ctb_size) * ((c->height + ctb - 1) >> c->log2_ctb_size);
     const uint64_t u = samples / 16 + (c->chroma_format_idc == 3 ? luma / 16 : 0);
     uint64_t v = 4096 + (samples + (c->chroma_format_idc == 3 ? luma : 0)) * 2 + u * (16 + 16 + 32 + 16 + 32) + (uint64_t)L.total * 2 + nctb * 3 * 16 +
-                 (samples >> 4) /* CIP + TQB bitmaps */ + luma / 16 * 4 + luma / 64 + luma / 16 + nctb * 2 /* DBD: leaves, QP, PCM, offsets */ + nctb * 4 + 4 /* intra CTB index */ + (1u << 20);
+                 (samples >> 4) /* CIP + TQB bitmaps */ + luma / 16 * 4 + luma / 64 + luma / 16 + nctb * 2 /* DBD: leaves, QP, PCM, offsets */ + (1u << 20);
     if (c->max_blob_bytes && c->max_blob_bytes < v) v = c->max_blob_bytes;
     return (v + 4095) & ~(uint64_t)4095;
 }
@@ -717,7 +637,7 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
         uint64_t need = b200_align_u32(r->off_pool + ((r->ncoef + 7) & ~7u) * 2, 256);
         for (int s = 0; s < 4; s++) need += ((uint64_t)r->tu[s].size() * 16 + 255) & ~(uint64_t)255;
         need += (((uint64_t)r->intra.size() * 16 + 255) & ~(uint64_t)255) + (((uint64_t)r->mc_count() * 32 + 255) & ~(uint64_t)255);
-        need += r->cip.size() * 4 + r->tqb.size() * 4 + r->dbd.size() * 4 + r->ccp.size() * sizeof(B200CcpRec) + 4 * ((size_t)r->ctb_w * r->ctb_h + 1) + 6 * 256;
+        need += r->cip.size() * 4 + r->tqb.size() * 4 + r->dbd.size() * 4 + r->ccp.size() * sizeof(B200CcpRec) + 5 * 256;
         if (rec_grow(r, need)) return B200_ENOMEM;
     }
     B200BlobHeader *h = (B200BlobHeader *)r->blob;
@@ -754,35 +674,14 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
         };
         std::stable_sort(r->intra.begin(), r->intra.end(), [&](const B200IntraRec &a, const B200IntraRec &b) { return key(a) < key(b); });
     }
-    bool ctb_order = false;
-    static thread_local std::vector<uint32_t> ictb;
     if (!r->intra.empty()) {
         static thread_local std::vector<uint32_t> perm;
-        static thread_local std::vector<uint8_t> lev;
-        // 1 (default): picture-wide level order, TU-granular wavefront (k_intra); 2: CTB order, CTB-granular stage (k_intra_ctb.cuh).
-        // The CTB-granular stage is bit-exact but has more serial steps: a CTB has up to ~80 dependency levels, and waiting for whole
-        // neighbour CTBs turns the ~3.4 k steps of the block-level graph of a 4K intra picture into ~10 k.
-        static const int intra_mode = getenv("B200_INTRA") ? atoi(getenv("B200_INTRA")) : 1;
         perm.resize(r->intra.size());
         B200IntraRec *dst = (B200IntraRec *)(r->blob + o);
-        const uint32_t nctb = (uint32_t)(r->ctb_w * r->ctb_h);
-        if (intra_mode == 2 && r->cip.empty()) {                 // (constrained_intra_pred pictures keep the TU-granular stage)
-            ictb.resize(nctb + 1); lev.resize(r->intra.size());
-            ctb_order = b200_intra_ctb_order(r->intra.data(), (uint32_t)r->intra.size(), r->cfg.width, r->cfg.height, r->cfg.chroma_format_idc,
-                                             r->cfg.log2_ctb_size, perm.data(), ictb.data(), lev.data()) >= 0;
-        }
-        if (ctb_order) for (size_t i = 0; i < perm.size(); i++) { dst[i] = r->intra[perm[i]]; dst[i].pad[0] = lev[i]; }
-        else {
-            b200_intra_level_order(r->intra.data(), (uint32_t)r->intra.size(), r->cfg.width, r->cfg.height, r->cfg.chroma_format_idc, perm.data());
-            for (size_t i = 0; i < perm.size(); i++) dst[i] = r->intra[perm[i]];
-        }
+        b200_intra_level_order(r->intra.data(), (uint32_t)r->intra.size(), r->cfg.width, r->cfg.height, r->cfg.chroma_format_idc, perm.data());
+        for (size_t i = 0; i < perm.size(); i++) dst[i] = r->intra[perm[i]];
     }
     o = (o + r->intra.size() * 16 + 255) & ~(uint64_t)255;
-    if (ctb_order) {                                         // CTB index of the intra list (k_intra_ctb.cuh)
-        h->ictb.off = (uint32_t)o; h->ictb.count = (uint32_t)ictb.size();
-        memcpy(r->blob + o, ictb.data(), ictb.size() * 4);
-        o = (o + ictb.size() * 4 + 255) & ~(uint64_t)255;
-    }
     h->sec[B200_SEC_MC].off = (uint32_t)o; h->sec[B200_SEC_MC].count = (uint32_t)r->mc_count();
     {   // big tiles first (decode order), then the <= 8x8 tiles bucketed by (chroma, bi): see B200BlobHeader.mc_big_count
         B200McRec *dst = (B200McRec *)(r->blob + o);

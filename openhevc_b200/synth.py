@@ -8,8 +8,6 @@ as exactly the records the recorder would produce for the same table calls.
 
 Host-side test / benchmark input generation only; nothing here computes reconstructed pixels.
 """
-import os
-
 import numpy as np
 
 from . import worklist as W
@@ -425,7 +423,6 @@ class FrameSynth:
                 self._quadtree(cx << self.log2_ctb, cy << self.log2_ctb, self.log2_ctb)
         pool, tu = self._coefficients()
         intra = np.zeros(len(self.intra), W.intra_dt)
-        ictb = None
         if self.intra:
             a = np.array(self.intra, np.int64)
             for k, name in enumerate(("plane", "x", "y", "log2", "mode", "flags", "top_right_size", "bottom_left_size")):
@@ -436,17 +433,9 @@ class FrameSynth:
             ro = a[:, 8]
             assert (ro != -2).all()
             intra["resid_off"] = np.where(ro < 0, W.NO_RESID, ro).astype(np.uint32)
-            # B200_INTRA=2: CTB order (CTB-granular stage, k_intra_ctb.cuh -- measured slower, see recorder.cpp); default (1): picture-wide
-            # dependency-level order (TU-granular stage).  constrained_intra_pred pictures always take the latter.
-            _, self.stats["intra_levels"] = W.level_order(intra, self.W, self.H, self.cfi)
-            co = None if (self.cip or os.environ.get("B200_INTRA", "1") != "2") else W.ctb_order(intra, self.W, self.H, self.cfi, self.log2_ctb)
-            if co is not None:
-                perm, ictb, lev, self.stats["intra_levels_in_ctb"] = co
-                intra = intra[perm]
-                intra["pad"][:, 0] = lev
-            else:
-                perm, _ = W.level_order(intra, self.W, self.H, self.cfi)
-                intra = intra[perm]
+            # picture-wide dependency-level order (the order k_intra takes the TUs in)
+            perm, self.stats["intra_levels"] = W.level_order(intra, self.W, self.H, self.cfi)
+            intra = intra[perm]
         mc = np.zeros(len(self.mc), W.mc_dt)
         if self.mc:
             for name in self.mc[0]:
@@ -455,7 +444,7 @@ class FrameSynth:
         dbk = self._deblock_grid() if self.deblock else None
         sao = self._sao_grid() if self.sao else None
         blob = W.build_blob(self.W, self.H, self.cfi, self.bd, self.log2_ctb, self.cur_slot, self.poc, pool, tu, intra, mc, dbk, sao, out=out,
-                            ref_slots=self.refs, cip=(2, self.is_intra) if self.cip else None, ictb=ictb)
+                            ref_slots=self.refs, cip=(2, self.is_intra) if self.cip else None)
         B = 2 if self.bd > 8 else 1
         S = sum(np.prod(W.plane_dims(self.W, self.H, self.cfi, p)) for p in range(3))
         st = self.stats

@@ -24,7 +24,7 @@ header_dt = np.dtype([
     ("width", "<u2"), ("height", "<u2"), ("chroma_format_idc", "u1"), ("bit_depth", "u1"),
     ("log2_ctb_size", "u1"), ("cur_slot", "u1"), ("flags", "<u4"),
     ("sec", section_dt, (SEC_COUNT,)), ("ref_slot", "u1", (16,)), ("n_ref", "u1"), ("pad", "u1", (3,)),
-    ("mc_big_count", "<u4"), ("cip", section_dt), ("tqb", section_dt), ("ccp", section_dt), ("dbd", section_dt), ("ictb", section_dt),
+    ("mc_big_count", "<u4"), ("cip", section_dt), ("tqb", section_dt), ("ccp", section_dt), ("dbd", section_dt), ("reserved_section", section_dt),
     ("reserved", "<u4", (64 - 23 - 2 * SEC_COUNT,)),
 ])
 tu_dt = np.dtype([("x", "<u2"), ("y", "<u2"), ("plane", "u1"), ("log2", "u1"), ("kind", "u1"), ("flags", "u1"),
@@ -133,25 +133,8 @@ def level_order(intra, width, height, cfi):
     return perm, rc
 
 
-def ctb_order(intra, width, height, cfi, log2_ctb):
-    """The order of the CTB-granular intra stage (b200_intra_ctb_order in libb200hevc.so, host code): (perm, ctb_start, levels, max level)
-    -- records grouped by CTB in raster order, inside a CTB by the dependency level counted inside the CTB -- or None when a CTB
-    has more than 255 levels (the caller keeps the picture-wide level order)."""
-    from . import _lib
-    lib = _lib.load()
-    intra = np.ascontiguousarray(intra, intra_dt)
-    nctb = ((width + (1 << log2_ctb) - 1) >> log2_ctb) * ((height + (1 << log2_ctb) - 1) >> log2_ctb)
-    perm = np.zeros(len(intra), np.uint32)
-    start = np.zeros(nctb + 1, np.uint32)
-    lev = np.zeros(len(intra), np.uint8)
-    rc = lib.b200_intra_ctb_order(intra.ctypes.data, len(intra), width, height, cfi, log2_ctb, perm.ctypes.data, start.ctypes.data, lev.ctypes.data)
-    if rc < 0:
-        return None
-    return perm, start, lev, rc
-
-
 def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=None, tu=None, intra=None, mc=None,
-               dbk=None, sao=None, out=None, ref_slots=(), cip=None, tqb=None, ictb=None):
+               dbk=None, sao=None, out=None, ref_slots=(), cip=None, tqb=None):
     """Assemble a blob.  tu: dict {2,3,4,5 -> tu_dt array}; dbk: uint16 array (DbkLayout.total) or None;
     sao: sao_dt array [3*ctb_count] or None.  `out`: optional uint8 buffer (e.g. pinned) to build into.
     cip: None, or (log2_min_pu, bool array [min_pu_height, min_pu_width], True = intra PU) for a constrained_intra_pred picture.
@@ -209,11 +192,6 @@ def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=N
                 if bitmap[cy * per:(cy + 1) * per, cx * per:(cx + 1) * per].any():
                     for pl in range(3):
                         g["tqb"][(pl * ch + cy) * cw + cx] = 1
-    if ictb is not None:                                   # CTB index of the intra list (B200BlobHeader.ictb)
-        ictb = np.ascontiguousarray(ictb, "<u4")
-        hdr["ictb"][0] = (off, len(ictb))
-        ictb_off = off
-        off = (off + ictb.nbytes + 255) // 256 * 256
     hdr["total_bytes"] = off
     if out is None:
         out = np.zeros(off, np.uint8)
@@ -230,8 +208,6 @@ def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=N
     if tqb_words is not None:
         o = int(hdr["tqb"][0]["off"])
         out[o:o + tqb_words.nbytes] = tqb_words.view(np.uint8)
-    if ictb is not None:
-        out[ictb_off:ictb_off + ictb.nbytes] = ictb.view(np.uint8)
     return out
 
 

@@ -4,7 +4,6 @@
 // 16x2 paths, tile / lane geometry and border rules are checked here, without a GPU.  Nothing in the product links this.
 #include "../../openhevc_b200/csrc/k_sao.cuh"
 #include "../../openhevc_b200/csrc/k_deblock.cuh"
-#include "../../openhevc_b200/csrc/k_mc.cuh"
 #include "../../openhevc_b200/csrc/k_intra_cip.cuh"
 #include <vector>
 
@@ -94,45 +93,5 @@ extern "C" int emul_cip_refs(const uint32_t *cip_words, const B200IntraRec *r, c
     cip_substitute(cd, cb, fl, r->bottom_left_size, top, left);
     for (int i = -1; i < 64; i++) { top65[i + 1] = top[i]; left65[i + 1] = left[i]; }
     *flags_out = fl & 31;
-    return 0;
-}
-
-// K1: the phases of k_mc.cuh in the order (and with the barriers, here: loop boundaries) of k_mc in kernels.cu.
-// dpb_planes[slot * 3 + plane]: host planes of the reference pictures (same pitches as the current picture);
-// ref_slot[i] = DPB slot of entry i of the picture's reference table.
-template <typename PIX, int GS>
-static void emul_mc_tile(const B200McRec *rec, const FrameDesc &cur, const std::vector<FrameDesc> &dpb, const uint8_t *ref_slot, int bd)
-{
-    alignas(16) uint16_t win[McSmem<GS>::WIN + 8];
-    alignas(16) int16_t tmp[McSmem<GS>::TMP + 8];
-    for (int i = 0; i < McSmem<GS>::WIN + 8; i++) win[i] = 0x5a5a;       // stale shared memory
-    for (int i = 0; i < McSmem<GS>::TMP + 8; i++) tmp[i] = 0x2b2b;
-    const int4 *rp4 = reinterpret_cast<const int4 *>(rec);
-    const McTile t = mc_decode<GS>(rp4[0], rp4[1]);
-    const bool chroma = t.flags & B200_MCF_CHROMA, bi = t.flags & B200_MCF_BI;
-    int v[2][GS][8];
-    for (int list = 0; list < 2; list++) {
-        if (list && !bi) break;
-        const PlaneDesc rp = dpb[ref_slot[list ? t.ref1 : t.ref0]].p[t.plane];
-        const int sx = list ? t.sx1 : t.sx0, sy = list ? t.sy1 : t.sy0, fr = list ? t.frac1 : t.frac0, mx = fr & 15, my = fr >> 4;
-        for (int gl = 0; gl < GS; gl++) { if (chroma) mc_load_window<PIX, 4, GS>(rp, t, sx, sy, mx, my, gl, win); else mc_load_window<PIX, 8, GS>(rp, t, sx, sy, mx, my, gl, win); }
-        if (mx)
-            for (int gl = 0; gl < GS; gl++) { if (chroma) mc_stage_a<4, GS>(t, sx, sy, mx, my, bd, gl, win, tmp); else mc_stage_a<8, GS>(t, sx, sy, mx, my, bd, gl, win, tmp); }
-        for (int gl = 0; gl < GS; gl++) { if (chroma) mc_stage_b<4, GS>(t, sx, sy, mx, my, bd, gl, win, tmp, v[list][gl]); else mc_stage_b<8, GS>(t, sx, sy, mx, my, bd, gl, win, tmp, v[list][gl]); }
-    }
-    for (int gl = 0; gl < GS; gl++) mc_store<PIX>(t, plane_of(cur, t.plane), bd, gl, v[0][gl], v[1][gl]);
-}
-
-extern "C" int emul_mc(const B200McRec *recs, int count, int n_big, uint8_t *const cur_planes[3], uint8_t *const *dpb_planes, int n_slots, const int pitch[3],
-                       int width, int height, int cfi, int bd, const uint8_t *ref_slot)
-{
-    FrameDesc cur;
-    describe(cur, cur_planes, pitch, width, height, cfi);
-    std::vector<FrameDesc> dpb(n_slots);
-    for (int s = 0; s < n_slots; s++) describe(dpb[s], dpb_planes + 3 * s, pitch, width, height, cfi);
-    for (int i = 0; i < count; i++) {
-        if (i < n_big) { if (bd > 8) emul_mc_tile<uint16_t, 32>(recs + i, cur, dpb, ref_slot, bd); else emul_mc_tile<uint8_t, 32>(recs + i, cur, dpb, ref_slot, bd); }
-        else           { if (bd > 8) emul_mc_tile<uint16_t, 8>(recs + i, cur, dpb, ref_slot, bd);  else emul_mc_tile<uint8_t, 8>(recs + i, cur, dpb, ref_slot, bd); }
-    }
     return 0;
 }

@@ -205,9 +205,9 @@ MC_CASES = [  # w, h, cfi, bd, kw
 
 @pytest.mark.parametrize("w,h,cfi,bd,kw", MC_CASES)
 def test_mc_phase_code_equals_oracle(emul, w, h, cfi, bd, kw):
-    """K1: the phases of k_mc.cuh (IDP.2A FIRs on packed pairs, interleaved row pairs between the passes) executed lane after
-    lane, against the oracle on pure inter pictures (every PU shape of the synthetic quadtrees, all 16 / 64 phases, uni / bi /
-    weighted, luma and chroma, windows hanging over the picture border)"""
+    """K1 (k_mc in kernels.cu, run by the warp-lockstep emulation with its group-local barriers: tests/emul/mc_emul.cpp) against
+    the oracle on pure inter pictures (every PU shape of the synthetic quadtrees, all 16 / 64 phases, uni / bi / weighted, luma
+    and chroma, windows hanging over the picture border, tiles of one warp and of 8-lane groups)"""
     from openhevc_b200.synth import FrameSynth, smooth_frame
     for seed in range(2):
         blob, st = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=800 + 10 * seed + bd + cfi, refs=[1, 2], cur_slot=0, p_intra=0.0, coded_frac=0.0,

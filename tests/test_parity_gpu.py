@@ -160,6 +160,9 @@ def test_malformed_blobs_are_rejected_not_executed():
             eng.submit(bad)
         with pytest.raises(B200Error):
             eng.submit(blob[:1000])
+        bad = blob.copy(); bad[:256].view(W.header_dt)["reserved_section"]["count"] = 1     # reserved header field in use
+        with pytest.raises(B200Error, match="reserved"):
+            eng.submit(bad)
         eng.decode(blob)                                        # context still usable
         # a record that points outside the picture / the coefficient pool / the reference table: caught by the
         # validation kernel in front of the picture's kernels (k_validate); the picture is not executed

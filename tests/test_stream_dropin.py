@@ -220,17 +220,6 @@ def test_two_decoders_in_one_process(threads):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", ["c1_832x480_i_16", "c2_1080p_ra8_65"])
-def test_ctb_granular_intra_stage_is_bit_exact(name):
-    """B200_INTRA=2: the CTB-granular intra stage (k_intra_ctb.cuh; not the default -- measured slower, DESIGN.md) on an all-intra
-    stream and on a random-access one"""
-    stream, md5 = os.path.join(RECIPE_DIR, name + ".hevc"), os.path.join(RECIPE_DIR, name + ".md5")
-    if not (os.path.exists(stream) and os.path.exists(md5) and os.path.exists(os.path.join(REFDIR, "decode_b200"))):
-        pytest.skip("recipe stream not generated (tools/make_bench_streams.sh)")
-    assert run("decode_b200", stream, 1, env={"B200_INTRA": "2"}) == open(md5).read().splitlines()
-
-
-@pytest.mark.gpu
 @pytest.mark.parametrize("env", [{"B200_MC": "4"}, {"B200_MC_SPLIT": "host"}, {"B200_DBD": "0"}, {"B200_DBD": "2"}], ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()))
 def test_switchable_paths_are_bit_exact_on_a_random_access_stream(env):
     """the paths behind environment switches, on the device: K1 with cp.async double buffering (B200_MC=4), prediction blocks cut into

@@ -32,7 +32,6 @@ def one(workload, lanes, pictures):
     for s in (W.SEC_TU4, W.SEC_TU4 + 1, W.SEC_TU4 + 2, W.SEC_TU4 + 3, W.SEC_INTRA, W.SEC_MC):
         hdr["sec"][0][s]["count"] = 0                      # the filters only: they run on whatever the slot holds
     hdr["mc_big_count"] = 0
-    hdr["ictb"][0]["count"] = 0
     pin = eng.pinned(blob.nbytes)
     pin[:blob.nbytes] = blob
     for s in range(n_slots):
