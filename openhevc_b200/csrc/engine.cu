@@ -467,62 +467,6 @@ static int check_blob(B200Ctx *ctx, const B200BlobHeader *h, uint64_t nbytes)
     return 0;
 }
 
-static int validate_mode()
-{
-    static const int mode = getenv("B200_VALIDATE") ? atoi(getenv("B200_VALIDATE")) : 1;   // 0 off, 1 device (default), 2 host
-    return mode;
-}
-
-// host-side validation (every record in range), on the submitting thread: B200_VALIDATE=2.  The default is the
-// same set of checks on the device (k_validate in kernels.cu) -- keep the two in step.
-static int deep_check(B200Ctx *ctx, const uint8_t *blob)
-{
-    const B200BlobHeader *h = (const B200BlobHeader *)blob;
-    const uint32_t ncoef = h->sec[B200_SEC_COEFF].count;
-    for (int s = B200_SEC_TU4; s <= B200_SEC_TU32; s++) {
-        const B200TuRec *t = (const B200TuRec *)(blob + h->sec[s].off);
-        const int n = 4 << (s - B200_SEC_TU4);
-        for (uint32_t i = 0; i < h->sec[s].count; i++) {
-            if (t[i].plane > 2 || (1 << t[i].log2) != n || t[i].x + n > ctx->pw[t[i].plane] || t[i].y + n > ctx->ph[t[i].plane] ||
-                (uint64_t)t[i].coeff_off + ((t[i].flags & B200_TUF_PARK) ? 2 : 0) + (t[i].nnz == B200_TU_DENSE ? n * n : 2 * (uint64_t)t[i].nnz) > ncoef ||
-                (t[i].nnz != B200_TU_DENSE && (int)t[i].nnz > n * n) || (t[i].kind == B200_TU_PCM && t[i].nnz != B200_TU_DENSE) ||
-                t[i].kind > B200_TU_PCM || (t[i].kind == B200_TU_DST && n != 4))
-                return fail(ctx, B200_EINVAL, "TU record %u of size %d invalid", i, n);
-        }
-    }
-    const B200IntraRec *ir = (const B200IntraRec *)(blob + h->sec[B200_SEC_INTRA].off);
-    for (uint32_t i = 0; i < h->sec[B200_SEC_INTRA].count; i++) {
-        const int n = 1 << ir[i].log2;
-        if (ir[i].plane > 2 || ir[i].log2 < 2 || ir[i].log2 > 5 || ir[i].mode > 34 || (ir[i].x & 3) || (ir[i].y & 3) ||
-            ir[i].x + n > ctx->pw[ir[i].plane] || ir[i].y + n > ctx->ph[ir[i].plane] ||
-            (ir[i].resid_off != B200_NO_RESID && ((uint64_t)ir[i].resid_off + n * n) * 2 > ctx->arena_bytes) ||
-            ((ir[i].flags & B200_INF_UP_RIGHT) && (ir[i].top_right_size < 1 || ir[i].top_right_size > n || ir[i].x + n + ir[i].top_right_size > ctx->pw[ir[i].plane])) ||
-            ((ir[i].flags & B200_INF_BOTTOM_LEFT) && (ir[i].bottom_left_size < 1 || ir[i].bottom_left_size > n || ir[i].y + n + ir[i].bottom_left_size > ctx->ph[ir[i].plane])) ||
-            ((ir[i].flags & (B200_INF_UP | B200_INF_UP_RIGHT | B200_INF_UP_LEFT)) && ir[i].y == 0) ||
-            ((ir[i].flags & (B200_INF_LEFT | B200_INF_BOTTOM_LEFT | B200_INF_UP_LEFT)) && ir[i].x == 0))
-            return fail(ctx, B200_EINVAL, "intra record %u invalid", i);
-    }
-    const B200McRec *mc = (const B200McRec *)(blob + h->sec[B200_SEC_MC].off);
-    const bool blocks = (h->mc_tile_count[0] | h->mc_tile_count[1] | h->mc_tile_count[2] | h->mc_tile_count[3] | h->mc_tile_count[4]) != 0;
-    for (uint32_t i = 0; i < h->sec[B200_SEC_MC].count; i++) {
-        const B200McRec &m = mc[i];
-        const int maxf = (m.flags & B200_MCF_CHROMA) ? 7 : 3;
-        if (blocks) {                                // whole prediction blocks (the device cuts them and validates the tiles again)
-            if (m.plane > 2 || !m.w || !m.h || m.w > 64 || m.h > 64 || m.x + m.w > ctx->pw[m.plane] || m.y + m.h > ctx->ph[m.plane] ||
-                m.ref0 >= h->n_ref || ((m.flags & B200_MCF_BI) && m.ref1 >= h->n_ref) ||
-                (m.frac0 & 15) > maxf || (m.frac0 >> 4) > maxf || (m.frac1 & 15) > maxf || (m.frac1 >> 4) > maxf || m.denom > 7)
-                return fail(ctx, B200_EINVAL, "MC block record %u invalid", i);
-            continue;
-        }
-        if (m.plane > 2 || !m.w || !m.h || m.w > 32 || m.w * m.h > 256 || m.x + m.w > ctx->pw[m.plane] || m.y + m.h > ctx->ph[m.plane] ||
-            m.ref0 >= h->n_ref || ((m.flags & B200_MCF_BI) && m.ref1 >= h->n_ref) ||
-            (m.frac0 & 15) > maxf || (m.frac0 >> 4) > maxf || (m.frac1 & 15) > maxf || (m.frac1 >> 4) > maxf || m.denom > 7 ||
-            ((m.w > 16) ? m.h > 8 : m.h > 16) || (i >= h->mc_big_count && !B200_MC_IS_SMALL(m.w, m.h)))
-            return fail(ctx, B200_EINVAL, "MC record %u invalid", i);
-    }
-    return 0;
-}
-
 // ---- slot hazards.  All calls come from the (single) submitting thread, in decode order, so "the event as recorded so
 // far" is exactly the set of earlier accesses.  `who`: lane index, RD_DOWN or RD_EXT. ----
 static int slot_acquire(B200Ctx *ctx, int slot, cudaStream_t st, int who, bool write)
@@ -573,10 +517,8 @@ extern "C" int b200_frame_upload(B200Ctx *ctx, const void *blob, uint64_t nbytes
     const B200BlobHeader *h = (const B200BlobHeader *)blob;
     int rc = check_blob(ctx, h, nbytes);
     if (rc) { ctx->err_code = 0; return rc; }
-    // every record is validated before it is used: by default on the device, in front of the picture's kernels
-    // (k_validate, a few microseconds; errors surface from b200_sync like the other device-side errors);
-    // B200_VALIDATE=2 checks on the host instead (synchronous error from this call), 0 = off
-    if (validate_mode() == 2 && (rc = deep_check(ctx, (const uint8_t *)blob))) { ctx->err_code = 0; return rc; }
+    // every record is validated before it is used: on the device, in front of the picture's kernels (k_validate, a few
+    // microseconds; errors surface from b200_sync like the other device-side errors)
     CU(cudaSetDevice(ctx->cfg.device));
     Arena &a = ctx->arena[arena];
     const void *src = blob;
@@ -681,7 +623,7 @@ extern "C" int b200_frame_execute_ex(B200Ctx *ctx, int arena, int cur_slot, cons
             mc_list = L.mc_tiles; mc_count = (uint32_t)tiles; mc_big = h.mc_tile_count[0];
         }
     }
-    if (validate_mode() == 1) ctx->launches += launch_validate(st, a.dev, h, ctx->pw, ctx->ph, ctx->arena_bytes, L.counter, mc_list == L.mc_tiles ? mc_list : nullptr, mc_count, mc_big);
+    ctx->launches += launch_validate(st, a.dev, h, ctx->pw, ctx->ph, ctx->arena_bytes, L.counter, mc_list == L.mc_tiles ? mc_list : nullptr, mc_count, mc_big);
     B200Ctx::TraceRec *tr = nullptr;
     if (ctx->trace_path && ctx->trace.size() < 4096) {
         ctx->trace.emplace_back();
@@ -693,8 +635,7 @@ extern "C" int b200_frame_execute_ex(B200Ctx *ctx, int arena, int cur_slot, cons
     }
     if (pf) CU(cudaEventRecord(ctx->prof[0], st));
     // K1 inter
-    ctx->launches += launch_mc(st, mc_list, (int)mc_count, (int)mc_big, cur, ctx->dpb_desc_dev, rt, bd, L.counter,
-                               ctx->slot_desc[0], (unsigned long long)ctx->slot_bytes);
+    ctx->launches += launch_mc(st, mc_list, (int)mc_count, (int)mc_big, cur, ctx->dpb_desc_dev, rt, bd, L.counter);
     if (pf) CU(cudaEventRecord(ctx->prof[1], st));
     if (tr) CU(cudaEventRecord(tr->ev[1], st));
     // K2 residual

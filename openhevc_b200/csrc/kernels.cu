@@ -472,19 +472,6 @@ __device__ __forceinline__ PlaneDesc ref_plane(const FrameDesc *__restrict__ dpb
 {
     return dpb[slot].p[plane];
 }
-// The DPB is one regular allocation (engine.cu: slot s starts at dpb + s * slot_bytes, same plane offsets in every slot), so a
-// reference plane can also be described from kernel parameters instead of being loaded from the descriptor table in global
-// memory -- one dependent memory latency less per list and tile (k_mc_v4).
-struct DpbLayout {
-    FrameDesc slot0;
-    unsigned long long slot_bytes;
-};
-__device__ __forceinline__ PlaneDesc ref_plane(const DpbLayout &L, int slot, int plane)
-{
-    PlaneDesc d = plane_of(L.slot0, plane);
-    d.base += (size_t)slot * L.slot_bytes;
-    return d;
-}
 
 struct McGeom {
     int w, h;
@@ -541,39 +528,10 @@ __device__ __forceinline__ uint32_t mc_ld_pair(const uint8_t *src)          // t
     return (t & 0xff) | ((t & 0xff00) << 8);
 }
 
-template <int TAPS, int GS, typename WT>
+// the FIRs of one list on a window that is complete in shared memory
+template <int TAPS, int GS>
 __device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
-                                            const WT *win, int16_t *tmp, int (&val)[8]);
-
-template <typename PIX, int TAPS, int GS>
-__device__ __forceinline__ void mc_list(const PlaneDesc &rp, int sx, int sy, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
-                                        uint16_t *win, int16_t *tmp, int (&val)[8])
-{
-    const McWin m = mc_win<TAPS>(sx, sy, mx, my, g);
-    const int R = m.R, np = m.np, ax = m.ax, oy = m.oy;
-    __syncwarp(gmask);
-    if (mc_win_interior(m, rp)) {
-        // interior: one 2-sample load per lane, 1 or 2 rows per pass, no clamping
-        const int lpr = np <= GS / 2 ? GS / 2 : GS;         // lanes per window row
-        const int pi = gl & (lpr - 1), rsub = gl >= lpr ? 1 : 0, rstep = GS / lpr;
-        if (pi < np) {
-            const uint8_t *src = rp.base + (size_t)(oy + rsub) * rp.pitch + (size_t)(ax + 2 * pi) * sizeof(PIX);
-            uint32_t *dst = reinterpret_cast<uint32_t *>(win) + rsub * np + pi;
-            for (int r = rsub; r < R; r += rstep) {
-                *dst = mc_ld_pair<PIX>(src);
-                src += (size_t)rstep * rp.pitch; dst += rstep * np;
-            }
-        }
-    } else mc_win_clamped<PIX, GS>(m, rp, gl, win);
-    __syncwarp(gmask);
-    mc_list_fir<TAPS, GS>(m, mx, my, g, bd, gl, gmask, win, tmp, val);
-}
-
-// the FIRs of one list on a window that is complete in shared memory (WT: uint16_t, or the picture's own sample type for the
-// windows k_mc_v4 copies asynchronously)
-template <int TAPS, int GS, typename WT>
-__device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, const McGeom &g, int bd, int gl, unsigned gmask,
-                                            const WT *win, int16_t *tmp, int (&val)[8])
+                                            const uint16_t *win, int16_t *tmp, int (&val)[8])
 {
     const int R = m.R, Ws = m.Ws, skew = m.skew;
     const int8_t *fxp = TAPS == 8 ? c_qpel[mx] : c_epel[mx];
@@ -587,7 +545,7 @@ __device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, cons
         if (qi < g.q) {
             const int sh = bd - 8;
             for (int r = gl >> g.lsh; r < R; r += rstep) {
-                const WT *s = win + r * Ws + skew + 4 * qi;
+                const uint16_t *s = win + r * Ws + skew + 4 * qi;
                 int p[TAPS + 3];
 #pragma unroll
                 for (int k = 0; k < TAPS + 3; k++) p[k] = s[k];
@@ -616,7 +574,7 @@ __device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, cons
 #pragma unroll
         for (int k = 0; k < 8 + TAPS - 1; k++) a[k] = s[k * g.ts];
     } else {
-        const WT *s = win + y0 * Ws + skew + xl;
+        const uint16_t *s = win + y0 * Ws + skew + xl;
 #pragma unroll
         for (int k = 0; k < 8 + TAPS - 1; k++) a[k] = s[k * Ws];
     }
@@ -639,7 +597,6 @@ __device__ __forceinline__ void mc_list_fir(const McWin &m, int mx, int my, cons
     }
 }
 
-// ---- K1, default version (k_mc): scalar FIRs (one IMAD per tap) ----
 // B200McRec fields straight from the two 16-byte halves of the record
 struct McRec {
     int dx, dy, w, h, plane, flags, sx0, sy0, sx1, sy1, ref0, ref1, frac0, frac1, w0, w1, o0, o1, denom;
@@ -707,44 +664,13 @@ __device__ __forceinline__ void mc_store(const McRec &t, const McGeom &g, const 
     }
 }
 
+// The window loads of BOTH lists are issued before anything waits for them.  Fetching a window in passes of a few 4-byte loads
+// per lane, and the second list only after the first has been filtered, costs several dependent round trips to L2 / HBM per
+// bi-predicted tile in a stage that waits on exactly those loads (long scoreboard, DRAM at 10 %).  Here a lane issues up to
+// 2 x 15 loads back to back into registers, then commits them to the two shared-memory windows.
+#define MC_PASSES 15          // 32x8 tiles: 15 rows, one per pass; 16x16 tiles: 23 rows, two per pass; 8-lane groups: <= 15 rows
 template <typename PIX, int GS>
-__global__ void __launch_bounds__(256) k_mc(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                         const uint32_t *__restrict__ gate)
-{
-    if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
-    constexpr int NG = 256 / GS;                           // groups per CTA
-    __shared__ __align__(16) uint16_t win_s[NG][McSmem<GS>::WIN];
-    __shared__ __align__(16) int16_t tmp_s[NG][McSmem<GS>::TMP];
-    const int grp = threadIdx.x / GS, gl = threadIdx.x & (GS - 1);
-    const unsigned gmask = GS == 32 ? 0xffffffffu : (((1u << GS) - 1u) << ((threadIdx.x & 31) & ~(GS - 1)));
-    const int ri = blockIdx.x * NG + grp;
-    if (ri >= count) return;                               // whole groups leave: the barriers are group-local
-    const int4 *rp4 = reinterpret_cast<const int4 *>(recs + ri);
-    const McRec t = mc_rec<GS>(__ldg(rp4), __ldg(rp4 + 1));
-    const bool chroma = t.flags & B200_MCF_CHROMA, bi = t.flags & B200_MCF_BI;
-    const McGeom g = mc_geom<GS>(t.w, t.h);
-    int v0[8], v1[8];
-    {
-        const PlaneDesc rp = ref_plane(dpb, ref_slot_of(rt, t.ref0), t.plane);
-        if (chroma) mc_list<PIX, 4, GS>(rp, t.sx0, t.sy0, t.frac0 & 15, t.frac0 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v0);
-        else        mc_list<PIX, 8, GS>(rp, t.sx0, t.sy0, t.frac0 & 15, t.frac0 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v0);
-    }
-    if (bi) {
-        const PlaneDesc rp = ref_plane(dpb, ref_slot_of(rt, t.ref1), t.plane);
-        if (chroma) mc_list<PIX, 4, GS>(rp, t.sx1, t.sy1, t.frac1 & 15, t.frac1 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v1);
-        else        mc_list<PIX, 8, GS>(rp, t.sx1, t.sy1, t.frac1 & 15, t.frac1 >> 4, g, bd, gl, gmask, win_s[grp], tmp_s[grp], v1);
-    }
-    mc_store<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
-}
-
-// ---- K1, version 3 (B200_MC=3): the arithmetic of the default version, but the window loads of BOTH lists are issued before
-// anything waits for them.  The default version fetches a window in passes of four 4-byte loads per lane (the compiler's
-// unrolling of the row loop) and the second list only after the first has been filtered: six dependent round trips to L2 /
-// HBM per bi-predicted tile in a kernel that ncu shows waiting on exactly those loads (long scoreboard, DRAM at 10 %).
-// Here a lane issues up to 2 x 15 loads back to back into registers, then commits them to the two shared-memory windows.
-#define MC3_PASSES 15          // 32x8 tiles: 15 rows, one per pass; 16x16 tiles: 23 rows, two per pass; 8-lane groups: <= 15 rows
-template <typename PIX, int GS>
-__device__ __forceinline__ void mc3_issue(const McWin &m, const PlaneDesc &rp, int gl, uint32_t (&v)[MC3_PASSES])
+__device__ __forceinline__ void mc_issue(const McWin &m, const PlaneDesc &rp, int gl, uint32_t (&v)[MC_PASSES])
 {
     const int np = m.np;
     const int lpr = np <= GS / 2 ? GS / 2 : GS;         // lanes per window row
@@ -753,10 +679,10 @@ __device__ __forceinline__ void mc3_issue(const McWin &m, const PlaneDesc &rp, i
     // loop is straight-line code and every load is in flight before the first one is needed
     const uint8_t *src = rp.base + (size_t)m.oy * rp.pitch + (size_t)(m.ax + 2 * pi) * sizeof(PIX);
 #pragma unroll
-    for (int i = 0; i < MC3_PASSES; i++) v[i] = mc_ld_pair<PIX>(src + (size_t)min(rsub + i * rstep, m.R - 1) * rp.pitch);
+    for (int i = 0; i < MC_PASSES; i++) v[i] = mc_ld_pair<PIX>(src + (size_t)min(rsub + i * rstep, m.R - 1) * rp.pitch);
 }
 template <typename PIX, int GS>
-__device__ __forceinline__ void mc3_commit(const McWin &m, const PlaneDesc &rp, int gl, const uint32_t (&v)[MC3_PASSES], uint16_t *win)
+__device__ __forceinline__ void mc_commit(const McWin &m, const PlaneDesc &rp, int gl, const uint32_t (&v)[MC_PASSES], uint16_t *win)
 {
     const int np = m.np;
     const int lpr = np <= GS / 2 ? GS / 2 : GS;
@@ -764,16 +690,16 @@ __device__ __forceinline__ void mc3_commit(const McWin &m, const PlaneDesc &rp, 
     if (pi >= np) return;
     uint32_t *dst = reinterpret_cast<uint32_t *>(win) + rsub * np + pi;
 #pragma unroll
-    for (int i = 0; i < MC3_PASSES; i++)
+    for (int i = 0; i < MC_PASSES; i++)
         if (rsub + i * rstep < m.R) dst[i * rstep * np] = v[i];
     // taller windows than any valid tile produces (the validation kernel bounds w and h): finish row by row
-    for (int r = rsub + MC3_PASSES * rstep; r < m.R; r += rstep)
+    for (int r = rsub + MC_PASSES * rstep; r < m.R; r += rstep)
         dst[(r - rsub) * np] = mc_ld_pair<PIX>(rp.base + (size_t)(m.oy + r) * rp.pitch + (size_t)(m.ax + 2 * pi) * sizeof(PIX));
 }
 
 template <typename PIX, int GS>
-__global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
-                                            const uint32_t *__restrict__ gate)
+__global__ void __launch_bounds__(256, 3) k_mc(const B200McRec *__restrict__ recs, int count, FrameDesc cur, const FrameDesc *__restrict__ dpb, RefTable rt, int bd,
+                                         const uint32_t *__restrict__ gate)
 {
     if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
     constexpr int NG = 256 / GS;                           // groups per CTA
@@ -794,13 +720,13 @@ __global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ 
     const McWin m1 = chroma ? mc_win<4>(t.sx1, t.sy1, mx1, my1, g) : mc_win<8>(t.sx1, t.sy1, mx1, my1, g);
     const bool in0 = mc_win_interior(m0, rp0), in1 = bi && mc_win_interior(m1, rp1);      // uniform over the group
     uint16_t *win0 = win_s[grp][0], *win1 = win_s[grp][1];
-    uint32_t r0[MC3_PASSES], r1[MC3_PASSES];
-    if (in0) mc3_issue<PIX, GS>(m0, rp0, gl, r0);
-    if (in1) mc3_issue<PIX, GS>(m1, rp1, gl, r1);
+    uint32_t r0[MC_PASSES], r1[MC_PASSES];
+    if (in0) mc_issue<PIX, GS>(m0, rp0, gl, r0);
+    if (in1) mc_issue<PIX, GS>(m1, rp1, gl, r1);
     if (!in0) mc_win_clamped<PIX, GS>(m0, rp0, gl, win0);
     if (bi && !in1) mc_win_clamped<PIX, GS>(m1, rp1, gl, win1);
-    if (in0) mc3_commit<PIX, GS>(m0, rp0, gl, r0, win0);
-    if (in1) mc3_commit<PIX, GS>(m1, rp1, gl, r1, win1);
+    if (in0) mc_commit<PIX, GS>(m0, rp0, gl, r0, win0);
+    if (in1) mc_commit<PIX, GS>(m1, rp1, gl, r1, win1);
     __syncwarp(gmask);
     int v0[8], v1[8];
     if (chroma) mc_list_fir<4, GS>(m0, mx0, my0, g, bd, gl, gmask, win0, tmp_s[grp], v0);
@@ -811,141 +737,6 @@ __global__ void __launch_bounds__(256, 3) k_mc_v3(const B200McRec *__restrict__ 
         else        mc_list_fir<8, GS>(m1, mx1, my1, g, bd, gl, gmask, win1, tmp_s[grp], v1);
     }
     mc_store<PIX>(t, g, plane_of(cur, t.plane), bd, gl, v0, v1);
-}
-
-
-// ---- K1, version 4 (B200_MC=4): the arithmetic of the default version behind a software pipeline.  ncu on versions 1 and 3: the
-// stage waits for its window loads (long scoreboard 9 per issue, DRAM at 10 %); a tile pays record -> descriptor -> window as
-// dependent round trips, in 4-byte loads, and nothing overlaps them.  Here the groups are PERSISTENT: while a group filters
-// tile k from one shared-memory buffer, the windows of both lists of tile k + 1 arrive in the other one through 16-byte
-// asynchronous copies (cp.async: LDGSTS.E.128, no register staging), and the record of tile k + 2 is already in registers.
-// Windows are kept in the picture's own sample type with rows of whole 16-byte chunks (the origin aligned down to a chunk:
-// `skew`); tiles whose window leaves the picture take the clamped, synchronous fill (emulated_edge_mc semantics, ~2 % of tiles).
-// Reference planes are described from kernel parameters (DpbLayout): no descriptor load in the pipeline.
-#ifndef B200_EMUL
-__device__ __forceinline__ void cp_async16(void *dst_smem, const void *src)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-#else
-static inline void cp_async16(void *dst, const void *src) { memcpy(dst, src, 16); }
-static inline void cp_async_commit() {}
-template <int N> static inline void cp_async_wait() {}
-#endif
-
-template <int GS> struct Mc4Smem;
-template <> struct Mc4Smem<32> { static constexpr int WIN_BYTES = 1536, TMP = MC_TMP_MAX, THREADS = 256; };   // (16+7) rows x 4 chunks, 15 rows x 6 chunks
-template <> struct Mc4Smem<8>  { static constexpr int WIN_BYTES = 768,  TMP = 128,        THREADS = 128; };   // 15 rows x 3 chunks
-
-// window of one list of one tile in the chunked layout (fields named like McWin: the FIR code is shared)
-template <typename PIX, int TAPS>
-__device__ __forceinline__ McWin mc4_win(int sx, int sy, int mx, int my, const McGeom &g, const PlaneDesc &rp, bool &interior)
-{
-    constexpr int BEFORE = TAPS == 8 ? 3 : 1, SPC = 16 / (int)sizeof(PIX);
-    McWin m;
-    const int C = g.w + (mx ? TAPS - 1 : 0);
-    m.R = g.h + (my ? TAPS - 1 : 0);
-    m.ox = sx - (mx ? BEFORE : 0); m.oy = sy - (my ? BEFORE : 0);
-    interior = m.ox >= 0 && m.oy >= 0 && m.ox + C <= rp.w && m.oy + m.R <= rp.h;
-    if (interior) {
-        m.skew = m.ox & (SPC - 1); m.ax = m.ox - m.skew;
-        m.np = (C + m.skew + SPC - 1) / SPC;                 // chunks per row
-        m.Ws = m.np * SPC;
-    } else {
-        m.skew = 0; m.ax = m.ox; m.np = 0;
-        m.Ws = (C + 1) & ~1;
-    }
-    return m;
-}
-template <typename PIX, int GS>
-__device__ __forceinline__ void mc4_fill(const McWin &m, bool interior, const PlaneDesc &rp, int gl, PIX *win)
-{
-    constexpr int SPC = 16 / (int)sizeof(PIX);
-    if (interior) {
-        const int total = m.R * m.np;
-        const uint8_t *base = rp.base + (size_t)m.oy * rp.pitch + (size_t)m.ax * sizeof(PIX);
-        for (int q = gl; q < total; q += GS) {
-            const int r = q / m.np, c = q - r * m.np;
-            cp_async16(win + r * m.Ws + c * SPC, base + (size_t)r * rp.pitch + 16 * c);
-        }
-    } else {
-        for (int i = gl; i < m.R * m.Ws; i += GS) {
-            const int r = i / m.Ws, cc = i - r * m.Ws;
-            const int x = clip3i(m.ax + cc, 0, rp.w - 1), y = clip3i(m.oy + r, 0, rp.h - 1);
-            win[i] = __ldg(px_ptr<PIX>(rp, x, y));
-        }
-    }
-}
-
-template <typename PIX, int GS>
-__global__ void __launch_bounds__(Mc4Smem<GS>::THREADS) k_mc_v4(const B200McRec *__restrict__ recs, int count, FrameDesc cur, RefTable rt, int bd, const uint32_t *__restrict__ gate,
-                                                               DpbLayout lay)
-{
-    if (__ldg(gate + 1)) return;         // the picture's work list failed validation (k_validate)
-    constexpr int THREADS = Mc4Smem<GS>::THREADS, NG = THREADS / GS, WB = Mc4Smem<GS>::WIN_BYTES;
-#ifdef B200_EMUL
-    static __align__(16) uint8_t smem[NG * (4 * WB + Mc4Smem<GS>::TMP * 2)];
-#else
-    extern __shared__ __align__(16) uint8_t smem[];
-#endif
-    const int grp = threadIdx.x / GS, gl = threadIdx.x & (GS - 1);
-    const unsigned gmask = GS == 32 ? 0xffffffffu : (((1u << GS) - 1u) << ((threadIdx.x & 31) & ~(GS - 1)));
-    uint8_t *wbase = smem + (size_t)grp * 4 * WB;                                   // [buffer][list]
-    int16_t *tmp = reinterpret_cast<int16_t *>(smem + (size_t)NG * 4 * WB) + grp * Mc4Smem<GS>::TMP;
-    const int stride = gridDim.x * NG;
-    int ti = blockIdx.x * NG + grp;
-    if (ti >= count) return;                                                        // whole groups leave: the barriers are group-local
-
-    struct Tile { McRec t; McGeom g; McWin m0, m1; bool bi, chroma; };
-    auto decode = [&](const int4 ra, const int4 rb) {
-        Tile T;
-        T.t = mc_rec<GS>(ra, rb);
-        T.chroma = T.t.flags & B200_MCF_CHROMA; T.bi = T.t.flags & B200_MCF_BI;
-        T.g = mc_geom<GS>(T.t.w, T.t.h);
-        return T;
-    };
-    auto issue = [&](Tile &T, int buf) {                                            // windows of both lists -> buffer `buf`
-        const PlaneDesc rp0 = ref_plane(lay, ref_slot_of(rt, T.t.ref0), T.t.plane);
-        bool in0, in1 = false;
-        T.m0 = T.chroma ? mc4_win<PIX, 4>(T.t.sx0, T.t.sy0, T.t.frac0 & 15, T.t.frac0 >> 4, T.g, rp0, in0) : mc4_win<PIX, 8>(T.t.sx0, T.t.sy0, T.t.frac0 & 15, T.t.frac0 >> 4, T.g, rp0, in0);
-        mc4_fill<PIX, GS>(T.m0, in0, rp0, gl, reinterpret_cast<PIX *>(wbase + (size_t)(2 * buf) * WB));
-        if (T.bi) {
-            const PlaneDesc rp1 = ref_plane(lay, ref_slot_of(rt, T.t.ref1), T.t.plane);
-            T.m1 = T.chroma ? mc4_win<PIX, 4>(T.t.sx1, T.t.sy1, T.t.frac1 & 15, T.t.frac1 >> 4, T.g, rp1, in1) : mc4_win<PIX, 8>(T.t.sx1, T.t.sy1, T.t.frac1 & 15, T.t.frac1 >> 4, T.g, rp1, in1);
-            mc4_fill<PIX, GS>(T.m1, in1, rp1, gl, reinterpret_cast<PIX *>(wbase + (size_t)(2 * buf + 1) * WB));
-        }
-    };
-
-    const int4 *rp4 = reinterpret_cast<const int4 *>(recs);
-    Tile cur_t = decode(__ldg(rp4 + 2 * (size_t)ti), __ldg(rp4 + 2 * (size_t)ti + 1));
-    issue(cur_t, 0);
-    cp_async_commit();
-    int4 na = make_int4(0, 0, 0, 0), nb = na;
-    if (ti + stride < count) { na = __ldg(rp4 + 2 * (size_t)(ti + stride)); nb = __ldg(rp4 + 2 * (size_t)(ti + stride) + 1); }
-    for (int it = 0; ti < count; ti += stride, it++) {
-        const bool has_next = ti + stride < count;
-        Tile next_t = cur_t;
-        if (has_next) { next_t = decode(na, nb); issue(next_t, (it + 1) & 1); }
-        cp_async_commit();
-        if (ti + 2 * stride < count) { na = __ldg(rp4 + 2 * (size_t)(ti + 2 * stride)); nb = __ldg(rp4 + 2 * (size_t)(ti + 2 * stride) + 1); }
-        cp_async_wait<1>();                                                         // this tile's windows have landed (the next tile's may not)
-        __syncwarp(gmask);
-        const PIX *w0 = reinterpret_cast<const PIX *>(wbase + (size_t)(2 * (it & 1)) * WB), *w1 = reinterpret_cast<const PIX *>(wbase + (size_t)(2 * (it & 1) + 1) * WB);
-        const McRec &t = cur_t.t;
-        int v0[8], v1[8];
-        if (cur_t.chroma) mc_list_fir<4, GS>(cur_t.m0, t.frac0 & 15, t.frac0 >> 4, cur_t.g, bd, gl, gmask, w0, tmp, v0);
-        else              mc_list_fir<8, GS>(cur_t.m0, t.frac0 & 15, t.frac0 >> 4, cur_t.g, bd, gl, gmask, w0, tmp, v0);
-        if (cur_t.bi) {
-            __syncwarp(gmask);                                                      // list 0's second pass has read tmp
-            if (cur_t.chroma) mc_list_fir<4, GS>(cur_t.m1, t.frac1 & 15, t.frac1 >> 4, cur_t.g, bd, gl, gmask, w1, tmp, v1);
-            else              mc_list_fir<8, GS>(cur_t.m1, t.frac1 & 15, t.frac1 >> 4, cur_t.g, bd, gl, gmask, w1, tmp, v1);
-        }
-        mc_store<PIX>(t, cur_t.g, plane_of(cur, t.plane), bd, gl, v0, v1);
-        __syncwarp(gmask);                                                          // everybody is done with this buffer and tmp
-        cur_t = next_t;
-    }
 }
 
 
@@ -1471,74 +1262,28 @@ __global__ void k_fill(FrameDesc f, int value)
 // --------------------------------------------------------------------------------------------
 // launchers
 // --------------------------------------------------------------------------------------------
-static int sm_count()                    // SMs of the current device: the persistent grids below are sized per SM
+static int sm_count()                    // SMs of the current device: the persistent grid of K3 is sized per SM
 {
     int dev = 0, n = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     return n > 0 ? n : 1;
 }
-static void mc4_opt_in()               // more than 48 KB of dynamic shared memory per block: once per kernel
-{
-    static bool done = false;
-    if (done) return;
-    done = true;
-    cudaFuncSetAttribute(k_mc_v4<uint16_t, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(k_mc_v4<uint8_t, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(k_mc_v4<uint16_t, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(k_mc_v4<uint8_t, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-}
-static int mc4_grid(int blocks_needed)   // persistent blocks: a few per SM (B200_MC4_CTAS per SM, default 3), never more than the work
-{
-    static const int per_sm = getenv("B200_MC4_CTAS") ? atoi(getenv("B200_MC4_CTAS")) : 3;
-    const int cap = sm_count() * (per_sm > 0 ? per_sm : 3);
-    return blocks_needed < cap ? blocks_needed : cap;
-}
-
-int launch_mc(cudaStream_t st, const B200McRec *recs, int count, int n_big, const FrameDesc &cur, const FrameDesc *dpb_dev, const RefTable &rt, int bd, const uint32_t *gate,
-              const FrameDesc &slot0, unsigned long long slot_bytes)
+int launch_mc(cudaStream_t st, const B200McRec *recs, int count, int n_big, const FrameDesc &cur, const FrameDesc *dpb_dev, const RefTable &rt, int bd, const uint32_t *gate)
 {
     if (!count) return 0;
-    // 1 = scalar FIRs, one IMAD per tap (default, k_mc); 3 = the same arithmetic with the window loads of both lists issued back
-    // to back (k_mc_v3); 4 = persistent groups, windows double-buffered through 16-byte cp.async, descriptors from kernel
-    // parameters (k_mc_v4)
-    static const int version = getenv("B200_MC") ? atoi(getenv("B200_MC")) : 1;
-    DpbLayout lay4;
-    lay4.slot0 = slot0; lay4.slot_bytes = slot_bytes;
     int n = 0;
     const int n_small = count - n_big;
     if (n_big) {                        // one warp per tile
         const int grid = (n_big + 7) / 8;
-        if (version == 3) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
-        } else if (version == 4) {
-            constexpr int NG = Mc4Smem<32>::THREADS / 32, SM = NG * (4 * Mc4Smem<32>::WIN_BYTES + Mc4Smem<32>::TMP * 2);
-            mc4_opt_in();
-            const int g4 = mc4_grid((n_big + NG - 1) / NG);
-            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint16_t, 32>)(recs, n_big, cur, rt, bd, gate, lay4);
-            else        B200_LAUNCH(g4, Mc4Smem<32>::THREADS, SM, st, k_mc_v4<uint8_t, 32>)(recs, n_big, cur, rt, bd, gate, lay4);
-        } else {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
-        }
+        if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
+        else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 32>)(recs, n_big, cur, dpb_dev, rt, bd, gate);
         n++;
     }
     if (n_small) {                      // tiles of <= 8x8 samples: four per warp
         const int grid = (n_small + 31) / 32;
-        if (version == 3) {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc_v3<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
-        } else if (version == 4) {
-            constexpr int NG = Mc4Smem<8>::THREADS / 8, SM = NG * (4 * Mc4Smem<8>::WIN_BYTES + Mc4Smem<8>::TMP * 2);
-            mc4_opt_in();
-            const int g4 = mc4_grid((n_small + NG - 1) / NG);
-            if (bd > 8) B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint16_t, 8>)(recs + n_big, n_small, cur, rt, bd, gate, lay4);
-            else        B200_LAUNCH(g4, Mc4Smem<8>::THREADS, SM, st, k_mc_v4<uint8_t, 8>)(recs + n_big, n_small, cur, rt, bd, gate, lay4);
-        } else {
-            if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
-            else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
-        }
+        if (bd > 8) B200_LAUNCH(grid, 256, 0, st, k_mc<uint16_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
+        else        B200_LAUNCH(grid, 256, 0, st, k_mc<uint8_t, 8>)(recs + n_big, n_small, cur, dpb_dev, rt, bd, gate);
         n++;
     }
     return n;

@@ -25,13 +25,10 @@ struct B200Rec {
     uint32_t npark = 0;          // int16 used in the parked-residual pool
     std::vector<B200TuRec> tu[4];
     std::vector<B200IntraRec> intra;
-    // MC tiles, already in the buckets of the wire format: [0] tiles of any shape (one warp each), [1 + B200_MC_SMALL_KEY] tiles of
-    // <= 8x8 samples by (chroma, bi).  Plain arrays: this is the hottest append of the recorder (~10 tiles per prediction block).
-    struct McBucket { B200McRec *p = nullptr; size_t n = 0, cap = 0; } mcb[5];
-    size_t mc_count() const { return mcb[0].n + mcb[1].n + mcb[2].n + mcb[3].n + mcb[4].n; }
-    // B200_MC_SPLIT=device (default): whole prediction blocks travel (all in mcb[0], decode order) and the device cuts them into
-    // tiles; mc_tiles[] counts the tiles per bucket, a record's pad[] holds the index of its first tile in its bucket
-    bool mc_dev_split = true;
+    // MC: whole prediction blocks in decode order, which the device cuts into tiles (k_mc_expand).  mc_tiles[] counts the tiles
+    // per bucket of the wire format ([0] tiles of any shape, [1 + B200_MC_SMALL_KEY] tiles of <= 8x8 samples by (chroma, bi)); a
+    // block's pad[] holds the index of its first tile in its bucket.  A plain array: this is the hottest append of the recorder.
+    struct McBlocks { B200McRec *p = nullptr; size_t n = 0, cap = 0; } mcb;
     uint32_t mc_tiles[5] = { 0, 0, 0, 0, 0 };
     std::vector<uint32_t> cip;   // B200CipHeader + bitmap of a constrained_intra_pred picture (b200_rec_set_cip), else empty
     std::vector<B200CcpRec> ccp; // cross-component prediction records (b200_rec_ccp), executed between the residual and the intra stage
@@ -170,7 +167,6 @@ extern "C" int b200_rec_create(const B200Config *cfg, B200Rec **out)
     r->off_dbk = 256;
     r->off_sao = b200_align_u32(r->off_dbk + r->dbk.total * 2, 256);
     r->off_pool = b200_align_u32(r->off_sao + (uint32_t)(3 * r->ctb_w * r->ctb_h) * 16, 256);
-    r->mc_dev_split = !(getenv("B200_MC_SPLIT") && !strcmp(getenv("B200_MC_SPLIT"), "host"));
     r->cap_max = b200_worst_blob_bytes(cfg);
     r->cap = (r->off_pool + (r->cap_max >> 4) + (2u << 20) + 4095) & ~(uint64_t)4095;
     if (r->cap > r->cap_max) r->cap = r->cap_max;
@@ -186,7 +182,7 @@ extern "C" void b200_rec_destroy(B200Rec *r)
 {
     if (!r) return;
     if (r->pinned) b200_host_free(r->blob); else free(r->blob);
-    for (int k = 0; k < 5; k++) free(r->mcb[k].p);
+    free(r->mcb.p);
     delete r;
 }
 
@@ -195,7 +191,7 @@ extern "C" int b200_rec_begin(B200Rec *r, int cur_slot, int poc)
     if (!r || cur_slot < 0 || cur_slot > 255) return B200_EINVAL;
     memset(r->blob + r->off_sao, 0, r->off_pool - r->off_sao);            // the deblock grids (1 MB at 4K) are cleared by the first call that needs them
     for (int s = 0; s < 4; s++) r->tu[s].clear();
-    r->intra.clear(); for (int k = 0; k < 5; k++) { r->mcb[k].n = 0; r->mc_tiles[k] = 0; } r->cip.clear(); r->tqb.clear(); r->ccp.clear(); r->leaf.clear(); r->dbd.clear();
+    r->intra.clear(); r->mcb.n = 0; for (int k = 0; k < 5; k++) r->mc_tiles[k] = 0; r->cip.clear(); r->tqb.clear(); r->ccp.clear(); r->leaf.clear(); r->dbd.clear();
     r->ncoef = 0; r->npark = 0; r->any_dbk = r->any_sao = false;
     r->last_intra[0] = r->last_intra[1] = r->last_intra[2] = -1;
     r->cur_slot = cur_slot; r->poc = poc; r->open = true; r->nbytes = 0; r->n_ref = 0; r->merged = false;
@@ -364,9 +360,9 @@ extern "C" int b200_rec_intra(B200Rec *r, int plane, int x, int y, int log2, int
     return 0;
 }
 
-static inline int mc_bucket_push(B200Rec *r, int k, const B200McRec &t)
+static inline int mc_push(B200Rec *r, const B200McRec &t)
 {
-    B200Rec::McBucket &bk = r->mcb[k];
+    B200Rec::McBlocks &bk = r->mcb;
     if (bk.n == bk.cap) {
         const size_t cap = bk.cap ? 2 * bk.cap : 4096;
         B200McRec *np = (B200McRec *)realloc(bk.p, cap * sizeof(B200McRec));
@@ -399,8 +395,7 @@ extern "C" int b200_rec_mc(B200Rec *r, const B200McRec *b)
 {
     if (!r || !r->open || !b || b->plane > 2 || !b->w || !b->h || b->w > 64 || b->h > 64) return B200_EINVAL;
     if (b->x + b->w > r->pw[b->plane] || b->y + b->h > r->ph[b->plane]) return B200_EINVAL;
-    if (r->mc_dev_split) {
-        // the block travels whole; the device cuts it (k_mc_expand) exactly like the loop below
+    {   // the block travels whole; the device cuts it (k_mc_expand) exactly like the loop below
         int ntiles;
         const int k = mc_block_bucket(b->w, b->h, b->flags, &ntiles);
         if (k >= 0 && r->mc_tiles[k] + (uint32_t)ntiles < (1u << 24)) {
@@ -408,11 +403,12 @@ extern "C" int b200_rec_mc(B200Rec *r, const B200McRec *b)
             const uint32_t off = r->mc_tiles[k];
             t.pad[0] = (uint8_t)off; t.pad[1] = (uint8_t)(off >> 8); t.pad[2] = (uint8_t)(off >> 16);
             r->mc_tiles[k] += (uint32_t)ntiles;
-            return mc_bucket_push(r, 0, t);
+            return mc_push(r, t);
         }
     }
-    // split into tiles of <= 16 x 16 samples (blocks taller than 8 rows: the squarer tile has the smaller filter
-    // halo) or <= 32 x 8: one warp each on the device, tiles of <= 8 x 8 four per warp
+    // a block whose tiles differ in kind: every tile as a block of its own.  Tiles of <= 16 x 16 samples (blocks taller than
+    // 8 rows: the squarer tile has the smaller filter halo) or <= 32 x 8: one warp each on the device, tiles of <= 8 x 8 four
+    // per warp
     const int twmax = B200_MC_TILE_WMAX(b->h);
     for (int tx = 0; tx < b->w;) {
         const int tw = b->w - tx > twmax ? twmax : b->w - tx;
@@ -424,13 +420,9 @@ extern "C" int b200_rec_mc(B200Rec *r, const B200McRec *b)
             t.sx0 = (int16_t)(b->sx0 + tx); t.sy0 = (int16_t)(b->sy0 + ty);
             t.sx1 = (int16_t)(b->sx1 + tx); t.sy1 = (int16_t)(b->sy1 + ty);
             const int k = B200_MC_IS_SMALL(tw, th) ? 1 + B200_MC_SMALL_KEY(b->flags) : 0;
-            int rc;
-            if (r->mc_dev_split) {                       // (a block whose tiles differ in kind: every tile as a block of its own)
-                const uint32_t off = r->mc_tiles[k]++;
-                t.pad[0] = (uint8_t)off; t.pad[1] = (uint8_t)(off >> 8); t.pad[2] = (uint8_t)(off >> 16);
-                rc = mc_bucket_push(r, 0, t);
-            } else rc = mc_bucket_push(r, k, t);
-            if (rc) return rc;
+            const uint32_t off = r->mc_tiles[k]++;
+            t.pad[0] = (uint8_t)off; t.pad[1] = (uint8_t)(off >> 8); t.pad[2] = (uint8_t)(off >> 16);
+            if (int rc = mc_push(r, t)) return rc;
         }
         tx += tw;
     }
@@ -481,9 +473,9 @@ extern "C" int b200_rec_merge(B200Rec *d, B200Rec *s)
         if (ir.resid_off != B200_NO_RESID) ir.resid_off += pbase;
         d->intra.push_back(ir);
     }
-    for (int k = 0; k < 5; k++) {
-        B200Rec::McBucket &db = d->mcb[k];
-        const B200Rec::McBucket &sb = s->mcb[k];
+    {
+        B200Rec::McBlocks &db = d->mcb;
+        const B200Rec::McBlocks &sb = s->mcb;
         if (db.n + sb.n > db.cap) {
             const size_t cap = db.n + sb.n + 4096;
             B200McRec *np = (B200McRec *)realloc(db.p, cap * sizeof(B200McRec));
@@ -495,18 +487,16 @@ extern "C" int b200_rec_merge(B200Rec *d, B200Rec *s)
             if (m.ref0 >= s->n_ref || ((m.flags & B200_MCF_BI) && m.ref1 >= s->n_ref)) return B200_EINVAL;
             m.ref0 = map[m.ref0];
             if (m.flags & B200_MCF_BI) m.ref1 = map[m.ref1];
-            if (d->mc_dev_split) {                       // the block's tiles now follow the tiles d already has in that bucket
-                int nt;
-                const int bk = mc_block_bucket(m.w, m.h, m.flags, &nt);
-                if (bk < 0) return B200_EINVAL;
-                const uint32_t off = ((uint32_t)m.pad[0] | ((uint32_t)m.pad[1] << 8) | ((uint32_t)m.pad[2] << 16)) + d->mc_tiles[bk];
-                if (off + (uint32_t)nt >= (1u << 24)) return B200_ENOTSUP;
-                m.pad[0] = (uint8_t)off; m.pad[1] = (uint8_t)(off >> 8); m.pad[2] = (uint8_t)(off >> 16);
-            }
+            // the block's tiles now follow the tiles d already has in that bucket
+            int nt;
+            const int bk = mc_block_bucket(m.w, m.h, m.flags, &nt);
+            if (bk < 0) return B200_EINVAL;
+            const uint32_t off = ((uint32_t)m.pad[0] | ((uint32_t)m.pad[1] << 8) | ((uint32_t)m.pad[2] << 16)) + d->mc_tiles[bk];
+            if (off + (uint32_t)nt >= (1u << 24)) return B200_ENOTSUP;
+            m.pad[0] = (uint8_t)off; m.pad[1] = (uint8_t)(off >> 8); m.pad[2] = (uint8_t)(off >> 16);
             db.p[db.n++] = m;
         }
     }
-    if (d->mc_dev_split != s->mc_dev_split) return B200_EINVAL;
     for (int k = 0; k < 5; k++) d->mc_tiles[k] += s->mc_tiles[k];
     d->leaf.insert(d->leaf.end(), s->leaf.begin(), s->leaf.end());
     if (s->any_dbk) {
@@ -636,7 +626,7 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
     {   // room for the lists and the optional sections behind the pool, before any pointer into the blob is taken
         uint64_t need = b200_align_u32(r->off_pool + ((r->ncoef + 7) & ~7u) * 2, 256);
         for (int s = 0; s < 4; s++) need += ((uint64_t)r->tu[s].size() * 16 + 255) & ~(uint64_t)255;
-        need += (((uint64_t)r->intra.size() * 16 + 255) & ~(uint64_t)255) + (((uint64_t)r->mc_count() * 32 + 255) & ~(uint64_t)255);
+        need += (((uint64_t)r->intra.size() * 16 + 255) & ~(uint64_t)255) + (((uint64_t)r->mcb.n * 32 + 255) & ~(uint64_t)255);
         need += r->cip.size() * 4 + r->tqb.size() * 4 + r->dbd.size() * 4 + r->ccp.size() * sizeof(B200CcpRec) + 5 * 256;
         if (rec_grow(r, need)) return B200_ENOMEM;
     }
@@ -656,7 +646,7 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
     uint64_t o = b200_align_u32(r->off_pool + h->sec[B200_SEC_COEFF].count * 2, 256);
     uint64_t need = o;
     for (int s = 0; s < 4; s++) need += ((uint64_t)r->tu[s].size() * 16 + 255) & ~(uint64_t)255;
-    need += (((uint64_t)r->intra.size() * 16 + 255) & ~(uint64_t)255) + (((uint64_t)r->mc_count() * 32 + 255) & ~(uint64_t)255);
+    need += (((uint64_t)r->intra.size() * 16 + 255) & ~(uint64_t)255) + (((uint64_t)r->mcb.n * 32 + 255) & ~(uint64_t)255);
     if (need > r->cap) return B200_ENOMEM;
     for (int s = 0; s < 4; s++) {
         h->sec[B200_SEC_TU4 + s].off = (uint32_t)o; h->sec[B200_SEC_TU4 + s].count = (uint32_t)r->tu[s].size();
@@ -682,14 +672,12 @@ extern "C" int b200_rec_finish(B200Rec *r, const void **blob, uint64_t *nbytes)
         for (size_t i = 0; i < perm.size(); i++) dst[i] = r->intra[perm[i]];
     }
     o = (o + r->intra.size() * 16 + 255) & ~(uint64_t)255;
-    h->sec[B200_SEC_MC].off = (uint32_t)o; h->sec[B200_SEC_MC].count = (uint32_t)r->mc_count();
-    {   // big tiles first (decode order), then the <= 8x8 tiles bucketed by (chroma, bi): see B200BlobHeader.mc_big_count
-        B200McRec *dst = (B200McRec *)(r->blob + o);
-        for (int k = 0; k < 5; k++) { if (r->mcb[k].n) memcpy(dst, r->mcb[k].p, r->mcb[k].n * sizeof(B200McRec)); dst += r->mcb[k].n; }
-        h->mc_big_count = r->mc_dev_split ? 0 : (uint32_t)r->mcb[0].n;
-        if (r->mc_dev_split && r->mc_count()) for (int k = 0; k < 5; k++) h->mc_tile_count[k] = r->mc_tiles[k];
+    h->sec[B200_SEC_MC].off = (uint32_t)o; h->sec[B200_SEC_MC].count = (uint32_t)r->mcb.n;
+    if (r->mcb.n) {                                          // whole blocks: mc_big_count stays 0, the tile counts tell the device the cut
+        memcpy(r->blob + o, r->mcb.p, r->mcb.n * sizeof(B200McRec));
+        for (int k = 0; k < 5; k++) h->mc_tile_count[k] = r->mc_tiles[k];
     }
-    o = (o + r->mc_count() * 32 + 255) & ~(uint64_t)255;
+    o = (o + r->mcb.n * 32 + 255) & ~(uint64_t)255;
     if (!r->cip.empty()) {                                   // constrained_intra_pred picture: B200CipHeader + intra bitmap
         if (o + r->cip.size() * 4 + 256 > r->cap) return B200_ENOMEM;
         h->cip.off = (uint32_t)o; h->cip.count = (uint32_t)r->cip.size();

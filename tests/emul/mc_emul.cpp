@@ -22,8 +22,6 @@ extern "C" int emul_mc(const B200McRec *recs, int count, int n_big, uint8_t *con
     RefTable rt = { { 0, 0 } };
     for (int i = 0; i < 16; i++) rt.w[i >> 3] |= (uint64_t)ref_slot[i] << (8 * (i & 7));
     uint32_t gate[4] = { 0, 0, 0, 0 };                   // [1] != 0 would mean "work list rejected": the kernel then does nothing
-    // the planes here are separate host buffers, not one regular DPB allocation: the versions that read the descriptor table
-    // (default, B200_MC=3) only
-    launch_mc(nullptr, recs, count, n_big, cur, dpb.data(), rt, bd, gate, dpb[0], 0);
+    launch_mc(nullptr, recs, count, n_big, cur, dpb.data(), rt, bd, gate);
     return 0;
 }

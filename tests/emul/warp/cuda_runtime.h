@@ -174,8 +174,6 @@ cudaError_t cudaEventDestroy(cudaEvent_t e);
 static inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t = nullptr) { return cudaSuccess; }
 static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 static inline cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t, cudaEvent_t) { *ms = 0.f; return cudaSuccess; }
-enum { cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
-template <typename F> static inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }

@@ -220,11 +220,10 @@ def test_two_decoders_in_one_process(threads):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("env", [{"B200_MC": "4"}, {"B200_MC_SPLIT": "host"}, {"B200_DBD": "0"}, {"B200_DBD": "2"}], ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()))
+@pytest.mark.parametrize("env", [{"B200_DBD": "0"}, {"B200_DBD": "2"}], ids=lambda e: ",".join(f"{k}={v}" for k, v in e.items()))
 def test_switchable_paths_are_bit_exact_on_a_random_access_stream(env):
-    """the paths behind environment switches, on the device: K1 with cp.async double buffering (B200_MC=4), prediction blocks cut into
-    tiles on the host instead of by k_mc_expand, deblocking control recorded from the reference's own filter calls (B200_DBD=0) and
-    derived AND compared on the device (B200_DBD=2) -- 1920x1080 random access, 65 pictures, 4 frame threads"""
+    """the paths behind environment switches, on the device: deblocking control recorded from the reference's own filter calls
+    (B200_DBD=0) and derived AND compared on the device (B200_DBD=2) -- 1920x1080 random access, 65 pictures, 4 frame threads"""
     stream, md5 = os.path.join(RECIPE_DIR, "c2_1080p_ra8_65.hevc"), os.path.join(RECIPE_DIR, "c2_1080p_ra8_65.md5")
     if not (os.path.exists(stream) and os.path.exists(md5) and os.path.exists(os.path.join(REFDIR, "decode_b200"))):
         pytest.skip("recipe stream not generated (tools/make_bench_streams.sh)")

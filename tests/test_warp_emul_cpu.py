@@ -93,11 +93,10 @@ def test_golden_fixtures_on_the_emulated_kernels(emulated):
         test_golden.test_cuda_reproduces_reference_golden(path)
 
 
-# the experiments behind environment switches (read once per process, hence a child process each): bit-exact or not worth a GPU
-# visit.  B200_EMUL_ORDER changes the order in which the emulator runs the lanes between two collectives (reverse / shuffled):
+# environment switches (read once per process, hence a child process each): one compute lane, and other lane orders of the
+# emulator.  B200_EMUL_ORDER changes the order in which the emulator runs the lanes between two collectives (reverse / shuffled):
 # a kernel that needs a barrier it does not have passes in one order and fails in another.
-VARIANTS = [dict(B200_EMUL_ORDER="reverse"), dict(B200_EMUL_ORDER="random:7"), dict(B200_MC="3", B200_EMUL_ORDER="random:3"), dict(B200_MC="4"), dict(B200_MC="4", B200_EMUL_ORDER="reverse"),
-            dict(B200_VALIDATE="2", B200_LANES="1")]
+VARIANTS = [dict(B200_EMUL_ORDER="reverse"), dict(B200_EMUL_ORDER="random:7"), dict(B200_EMUL_ORDER="random:3"), dict(B200_LANES="1")]
 
 
 @needs_emul
