@@ -102,8 +102,8 @@ HD PIX *px_ptr(const PlaneDesc &p, int x, int y)
 
 // launchers (kernels.cu) -- all asynchronous on `st`; return number of kernels launched
 int launch_validate(cudaStream_t st, const uint8_t *blob_dev, const B200BlobHeader &h, const int pw[3], const int ph[3], unsigned long long arena_bytes, uint32_t *gate,
-                    const B200McRec *mc_tiles = nullptr, uint32_t mc_count = 0, uint32_t mc_big = 0);
-int launch_mc_expand(cudaStream_t st, const B200McRec *blocks, uint32_t n_blocks, B200McRec *tiles, const uint32_t count[5], uint32_t *gate);
+                    const B200McRec *mc_tiles = nullptr, uint32_t mc_count = 0, uint32_t mc_big = 0, uint32_t mc_tag = 0);
+int launch_mc_expand(cudaStream_t st, const B200McRec *blocks, uint32_t n_blocks, B200McRec *tiles, const uint32_t count[5], uint32_t tag, uint32_t *gate);
 int launch_mc(cudaStream_t st, const B200McRec *recs, int count, int n_big, const FrameDesc &cur, const FrameDesc *dpb_dev, const RefTable &rt, int bd, const uint32_t *gate);
 int launch_residual(cudaStream_t st, const B200TuRec *const recs[4], const int counts[4], const int16_t *pool, int16_t *parked, const FrameDesc &cur, int bd, const uint32_t *gate);
 int launch_ccp(cudaStream_t st, const B200CcpRec *recs, int count, int16_t *parked, const FrameDesc &cur, int bd, uint32_t *gate, unsigned long long arena_bytes);

@@ -56,9 +56,11 @@ struct Lane {
     uint8_t *work = nullptr;            // pre-SAO picture (reconstruct + deblock happen here when the picture has SAO)
     FrameDesc work_desc;
     uint2 *flags[3] = { nullptr, nullptr, nullptr };   // intra edge records, 16 B per 4x4 unit
-    uint32_t *counter = nullptr;        // [0] K3 ticket, [1] validation gate of the picture in progress, [2] K3 time-out latch, [3] validation latch
+    uint32_t *counter = nullptr;        // [0] K3 ticket, [1] validation gate of the picture in progress, [2] K3 time-out latch, [3] validation latch,
+                                        // [6] tiles k_mc_expand wrote (kernels.cu)
     int16_t *parked = nullptr;          // residuals of intra TUs (K2 -> K3), indexed like the coefficient pool
     B200McRec *mc_tiles = nullptr;      // tile list k_mc_expand writes when the blob carries whole prediction blocks (B200BlobHeader.mc_tile_count)
+    uint32_t mc_tag = 0;                // stamp of the tiles k_mc_expand wrote for the lane's latest such picture (24 bits, never 0)
     DbdMaps dbd = {};                   // scratch of the on-device deblocking derivation, allocated with the first picture that needs it
     size_t dbd_bytes = 0;
     cudaEvent_t tail = nullptr;         // end of the last picture of this lane
@@ -618,12 +620,16 @@ extern "C" int b200_frame_execute_ex(B200Ctx *ctx, int arena, int cur_slot, cons
         uint64_t tiles = 0;
         for (int k = 0; k < 5; k++) tiles += h.mc_tile_count[k];
         if (tiles) {
-            if (!L.mc_tiles) CU(cudaMalloc(&L.mc_tiles, ctx->mc_tile_cap * sizeof(B200McRec)));
-            ctx->launches += launch_mc_expand(st, mc_list, mc_count, L.mc_tiles, h.mc_tile_count, L.counter);
+            const size_t bytes = ctx->mc_tile_cap * sizeof(B200McRec);
+            if (!L.mc_tiles) CU(cudaMalloc(&L.mc_tiles, bytes));
+            // a new stamp per picture; when the 24 bits run out (or on first use) no tile in the list may carry the next one
+            if (!L.mc_tag || L.mc_tag == 0xffffffu) { CU(cudaMemsetAsync(L.mc_tiles, 0, bytes, st)); L.mc_tag = 0; }
+            L.mc_tag++;
+            ctx->launches += launch_mc_expand(st, mc_list, mc_count, L.mc_tiles, h.mc_tile_count, L.mc_tag, L.counter);
             mc_list = L.mc_tiles; mc_count = (uint32_t)tiles; mc_big = h.mc_tile_count[0];
         }
     }
-    ctx->launches += launch_validate(st, a.dev, h, ctx->pw, ctx->ph, ctx->arena_bytes, L.counter, mc_list == L.mc_tiles ? mc_list : nullptr, mc_count, mc_big);
+    ctx->launches += launch_validate(st, a.dev, h, ctx->pw, ctx->ph, ctx->arena_bytes, L.counter, mc_list == L.mc_tiles ? mc_list : nullptr, mc_count, mc_big, L.mc_tag);
     B200Ctx::TraceRec *tr = nullptr;
     if (ctx->trace_path && ctx->trace.size() < 4096) {
         ctx->trace.emplace_back();

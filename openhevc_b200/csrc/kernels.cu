@@ -51,7 +51,7 @@ __host__ __device__ constexpr int hevc_T(int k, int n)
 // closes the picture's GATE (gate[1]): every kernel that consumes records returns at once, so a malformed list is
 // rejected, not executed; gate[3] latches the failing sections until b200_sync() reports them.
 // gate layout (uint32, one per compute lane): [0] K3 ticket, [1] gate of the picture in progress, [2] K3 time-out latch,
-// [3] validation latch.
+// [3] validation latch, [6] tiles k_mc_expand wrote for the picture in progress (k_validate compares and clears it).
 // --------------------------------------------------------------------------------------------
 // Error latches are mirrored into mapped host memory (engine.cu: gate[4..5] = device address of this lane's host word), so that
 // the host can notice a rejected picture without synchronising with the device (b200_poll_errors).
@@ -68,6 +68,7 @@ struct ValidateArgs {
     uint32_t ncoef, mc_big, n_ref;
     unsigned long long arena_bytes;
     const uint8_t *mc; uint32_t mc_count;      // the MC tile records: the blob's section, or the list k_mc_expand wrote
+    uint32_t mc_tag;                           // list k_mc_expand wrote: the stamp every tile of this picture carries; else 0
 };
 
 __global__ void __launch_bounds__(256) k_validate(ValidateArgs a, uint32_t *gate)
@@ -116,14 +117,22 @@ __global__ void __launch_bounds__(256) k_validate(ValidateArgs a, uint32_t *gate
         if (m.plane > 2 || !m.w || !m.h || m.w > 32 || m.w * m.h > 256 || m.x + m.w > pw || m.y + m.h > ph ||
             m.ref0 >= a.n_ref || ((m.flags & B200_MCF_BI) && m.ref1 >= a.n_ref) ||
             (m.frac0 & 15) > maxf || (m.frac0 >> 4) > maxf || (m.frac1 & 15) > maxf || (m.frac1 >> 4) > maxf || m.denom > 7 ||
-            ((m.w > 16) ? m.h > 8 : m.h > 16) || (i >= a.mc_big && !B200_MC_IS_SMALL(m.w, m.h)))
+            ((m.w > 16) ? m.h > 8 : m.h > 16) || (i >= a.mc_big && !B200_MC_IS_SMALL(m.w, m.h)) ||
+            (a.mc_tag && ((uint32_t)rb.w >> 8) != a.mc_tag))
             bad |= 1u << B200_SEC_MC;
+    }
+    // A place of the tile list that no block of this picture wrote still holds a tile of an earlier picture (without this
+    // picture's stamp, rejected above).  Every place stamped and as many tiles written as there are places: no place was
+    // written twice either, i.e. no two blocks claimed the same places.
+    if (i == 0 && a.mc_tag) {
+        if (gate[6] != a.mc_count) bad |= 1u << B200_SEC_MC;
+        gate[6] = 0;
     }
     if (bad) { gate[1] = 1u; atomicOr(gate + 3, bad); latch_host(gate, bad); }
 }
 
 int launch_validate(cudaStream_t st, const uint8_t *blob_dev, const B200BlobHeader &h, const int pw[3], const int ph[3], unsigned long long arena_bytes, uint32_t *gate,
-                    const B200McRec *mc_tiles, uint32_t mc_count, uint32_t mc_big)
+                    const B200McRec *mc_tiles, uint32_t mc_count, uint32_t mc_big, uint32_t mc_tag)
 {
     ValidateArgs a;
     a.blob = blob_dev;
@@ -133,6 +142,7 @@ int launch_validate(cudaStream_t st, const uint8_t *blob_dev, const B200BlobHead
     for (int s = 0; s < B200_SEC_COUNT; s++) { a.sec[s] = h.sec[s]; if (s >= B200_SEC_TU4 && s <= B200_SEC_INTRA && h.sec[s].count > most) most = h.sec[s].count; }
     for (int p = 0; p < 3; p++) { a.pw[p] = pw[p]; a.ph[p] = ph[p]; }
     a.ncoef = h.sec[B200_SEC_COEFF].count; a.mc_big = mc_tiles ? mc_big : h.mc_big_count; a.n_ref = h.n_ref; a.arena_bytes = arena_bytes;
+    a.mc_tag = mc_tiles ? mc_tag : 0;
     if (!most) return 0;
     B200_LAUNCH((most + 255) / 256, 256, 0, st, k_validate)(a, gate);
     return 1;
@@ -406,17 +416,19 @@ template <> struct McSmem<8>  { static constexpr int WIN = 256 /* 15 x 16 */, TM
 // coded picture): one thread per block writes the block's tiles -- the cut of B200_MC_TILE_WMAX / _HMAX, the one definition the
 // recorder's fallback uses too -- into the lane's tile list at the place the host reserved (bucket base + B200McRec.pad), laid
 // out like a B200_SEC_MC section in tile mode.  Only memory safety is checked here (index inside the bucket); the tiles are
-// validated like any other list by k_validate, which runs behind this kernel.
+// validated like any other list by k_validate, which runs behind this kernel.  Each tile carries the picture's stamp in its pad
+// bytes (k_mc reads no pad), and gate[6] counts the tiles written: with both, k_validate also rejects a list whose blocks leave
+// places of the tile list unwritten or claim the same places twice.
 struct McExpandArgs {
     const B200McRec *blocks; uint32_t n_blocks;
     B200McRec *tiles;
     uint32_t base[5], count[5];
+    uint32_t tag;                        // 24 bits, never 0
 };
 __global__ void __launch_bounds__(256) k_mc_expand(McExpandArgs a, uint32_t *gate)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= a.n_blocks) return;
-    const int4 *p = reinterpret_cast<const int4 *>(a.blocks) + 2 * (size_t)i;
+    const int4 *p = reinterpret_cast<const int4 *>(a.blocks) + 2 * (size_t)min(i, a.n_blocks - 1);
     const int4 ra = __ldg(p), rb = __ldg(p + 1);
     const int x = ra.x & 0xffff, y = (unsigned)ra.x >> 16, w = ra.y & 0xff, h = (ra.y >> 8) & 0xff, flags = (unsigned)ra.y >> 24;
     const int sx0 = (int16_t)(ra.z & 0xffff), sy0 = (int16_t)((unsigned)ra.z >> 16), sx1 = (int16_t)(ra.w & 0xffff), sy1 = (int16_t)((unsigned)ra.w >> 16);
@@ -424,7 +436,7 @@ __global__ void __launch_bounds__(256) k_mc_expand(McExpandArgs a, uint32_t *gat
     bool bad = !w || !h || w > 64 || h > 64;
     int bucket = -1;
     uint32_t k = 0;
-    if (!bad) {
+    if (i < a.n_blocks && !bad) {
         const int twmax = B200_MC_TILE_WMAX(h);
         for (int tx = 0; tx < w && !bad;) {
             const int tw = w - tx > twmax ? twmax : w - tx, maxh = B200_MC_TILE_HMAX(tw);
@@ -440,7 +452,7 @@ __global__ void __launch_bounds__(256) k_mc_expand(McExpandArgs a, uint32_t *gat
                 ta.y = (ra.y & 0xffff0000) | tw | (th << 8);
                 ta.z = ((sx0 + tx) & 0xffff) | ((sy0 + ty) << 16);
                 ta.w = ((sx1 + tx) & 0xffff) | ((sy1 + ty) << 16);
-                tb.w = rb.w & 0xff;                                       // denom; pad cleared
+                tb.w = (rb.w & 0xff) | (int)(a.tag << 8);                 // denom; pad = the picture's stamp
                 int4 *o = reinterpret_cast<int4 *>(a.tiles + bs + off + k);
                 o[0] = ta; o[1] = tb;
                 k++;
@@ -448,13 +460,17 @@ __global__ void __launch_bounds__(256) k_mc_expand(McExpandArgs a, uint32_t *gat
             tx += tw;
         }
     }
-    if (bad) { gate[1] = 1u; atomicOr(gate + 3, 1u << B200_SEC_MC); latch_host(gate, 1u << B200_SEC_MC); }
+    uint32_t n = k;                                                   // tiles written by the warp: one atomic per warp
+#pragma unroll
+    for (int s = 16; s; s >>= 1) n += __shfl_xor_sync(0xffffffffu, n, s);
+    if ((threadIdx.x & 31) == 0 && n) atomicAdd(gate + 6, n);
+    if (i < a.n_blocks && bad) { gate[1] = 1u; atomicOr(gate + 3, 1u << B200_SEC_MC); latch_host(gate, 1u << B200_SEC_MC); }
 }
-int launch_mc_expand(cudaStream_t st, const B200McRec *blocks, uint32_t n_blocks, B200McRec *tiles, const uint32_t count[5], uint32_t *gate)
+int launch_mc_expand(cudaStream_t st, const B200McRec *blocks, uint32_t n_blocks, B200McRec *tiles, const uint32_t count[5], uint32_t tag, uint32_t *gate)
 {
     if (!n_blocks) return 0;
     McExpandArgs a;
-    a.blocks = blocks; a.n_blocks = n_blocks; a.tiles = tiles;
+    a.blocks = blocks; a.n_blocks = n_blocks; a.tiles = tiles; a.tag = tag;
     uint32_t o = 0;
     for (int k = 0; k < 5; k++) { a.base[k] = o; a.count[k] = count[k]; o += count[k]; }
     B200_LAUNCH((n_blocks + 255) / 256, 256, 0, st, k_mc_expand)(a, gate);

@@ -38,7 +38,7 @@ static uint64_t rnd64(void) { uint64_t z = (g_seed += 0x9E3779B97F4A7C15ULL); z 
 static int rnd(int n) { return (int)(rnd64() % (uint64_t)n); }
 static int rndr(int lo, int hi) { return lo + rnd(hi - lo + 1); }
 
-static int g_fail, g_checks;
+static int g_fail, g_checks, g_wraps;
 #define CHECK(cond, ...) do { g_checks++; if (!(cond)) { if (g_fail < 20) { fprintf(stderr, "MISMATCH: " __VA_ARGS__); fprintf(stderr, "\n"); } g_fail++; } } while (0)
 
 /* native-format plane (uint8 for 8 bit, uint16 above) <-> oracle uint16 plane */
@@ -54,9 +54,23 @@ static Plane plane_alloc(int w, int h, int pad, int bd)
 static void plane_free(Plane *p) { free(p->base); }
 static void plane_put(Plane *p, int x, int y, int v) { if (p->bd > 8) ((uint16_t *)(p->data + y * p->stride))[x] = (uint16_t)v; else p->data[y * p->stride + x] = (uint8_t)v; }
 static int plane_get(const Plane *p, int x, int y) { return p->bd > 8 ? ((uint16_t *)(p->data + y * p->stride))[x] : p->data[y * p->stride + x]; }
-/* smooth-ish random content so that deblock / SAO / intra-strong decisions hit every branch */
+/* luma fraction 2 (hevcdsp.c:1028-1042): the 2-D filter of fraction (2, 2) has every tap product nonzero */
+static const int k_qpel2[8] = { -1, 4, -11, 40, 40, -11, 4, -1 };
+
+/* smooth-ish random content so that deblock / SAO / intra-strong decisions hit every branch; mode 2 (3): the sign pattern, the
+ * maximum where the tap product of fraction (2, 2) at (x mod 8, y mod 8) is positive (negative), else 0 -- the content that takes
+ * the 2-D intermediate to its maximum (minimum), beyond int16 for the maximum */
 static void plane_fill(Plane *p, int mode)
 {
+    if (mode >= 2) {
+        const int maxv = (1 << p->bd) - 1;
+        for (int y = -p->pad; y < p->h + p->pad; y++)
+            for (int x = -p->pad; x < p->w + p->pad; x++) {
+                const int prod = k_qpel2[x & 7] * k_qpel2[y & 7];
+                plane_put(p, x, y, (mode == 2 ? prod > 0 : prod < 0) ? maxv : 0);
+            }
+        return;
+    }
     int maxv = (1 << p->bd) - 1, base = rnd(maxv + 1), gx = rndr(-3, 3), gy = rndr(-3, 3), noise = mode == 0 ? maxv : (1 << rnd(4)) << (p->bd - 8);
     for (int y = -p->pad; y < p->h + p->pad; y++)
         for (int x = -p->pad; x < p->w + p->pad; x++) {
@@ -124,6 +138,24 @@ static void test_transforms(HEVCDSPContext *d, int bd, int trials)
 }
 
 /* ---------------------------------------------------------------- inter prediction */
+/* does the 2-D intermediate of luma fraction (2, 2) exceed int16 anywhere in the w x h block at (sx, sy)?  List 0 of a bi-predicted
+ * block travels through the int16 tmp[] of hevc.c:1761 and wraps there; the oracle must wrap it the same way */
+static int qpel22_exceeds_int16(const Plane *r, int sx, int sy, int w, int h, int bd)
+{
+    for (int y = 0; y < h; y++)
+        for (int x = 0; x < w; x++) {
+            int acc2 = 0;
+            for (int j = 0; j < 8; j++) {
+                const int yy = FFMIN(FFMAX(sy + y + j - 3, 0), r->h - 1);
+                int acc = 0;
+                for (int i = 0; i < 8; i++) acc += k_qpel2[i] * plane_get(r, FFMIN(FFMAX(sx + x + i - 3, 0), r->w - 1), yy);
+                acc2 += k_qpel2[j] * (acc >> (bd - 8));
+            }
+            if ((acc2 >> 6) > 32767) return 1;
+        }
+    return 0;
+}
+
 static void test_mc(HEVCDSPContext *d, VideoDSPContext *vd, int bd, int trials)
 {
     static const int widths[10] = { 2, 4, 6, 8, 12, 16, 24, 32, 48, 64 };
@@ -131,20 +163,24 @@ static void test_mc(HEVCDSPContext *d, VideoDSPContext *vd, int bd, int trials)
     for (int t = 0; t < trials; t++) {
         const int PW = 160, PH = 128;
         Plane r0 = plane_alloc(PW, PH, 0, bd), r1 = plane_alloc(PW, PH, 0, bd), dst = plane_alloc(PW, PH, 0, bd);
-        plane_fill(&r0, rnd(3) == 0); plane_fill(&r1, rnd(3) == 0); plane_fill(&dst, 1);
+        const int sign = rnd(4) == 0;              /* the sign pattern in list 0, its complement in list 1 */
+        plane_fill(&r0, sign ? 2 : rnd(3) == 0); plane_fill(&r1, sign ? 3 : rnd(3) == 0); plane_fill(&dst, 1);
         int chroma = rnd(2), widx = chroma ? rnd(9) : rndr(1, 9); if (!chroma && widths[widx] == 6) widx = 3;
         int w = widths[widx], h = chroma ? (1 + rnd(32)) * 2 : (1 + rnd(16)) * 4; if (h > 64) h = 64;
         int bi = rnd(2), weighted = rnd(2);
         int fmax = chroma ? 8 : 4, before = chroma ? 1 : 3, extra = chroma ? 3 : 7;
         int mx0 = rnd(fmax), my0 = rnd(fmax), mx1 = rnd(fmax), my1 = rnd(fmax);
+        if (sign && !chroma && bi) mx0 = my0 = 2;
         int dx = rnd(PW - w + 1), dy = rnd(PH - h + 1);
-        int edge = rnd(4) == 0;   /* let the source window hang over the picture: emulated_edge_mc path */
+        int edge = rnd(sign ? 8 : 4) == 0;   /* let the source window hang over the picture: emulated_edge_mc path */
         int sx[2], sy[2];
         for (int l = 0; l < 2; l++) {
             if (edge) { sx[l] = rndr(-w - 12, PW + 12); sy[l] = rndr(-h - 12, PH + 12); }
             else { sx[l] = rndr(before, PW - w - extra + before - 1); sy[l] = rndr(before, PH - h - extra + before - 1); }
         }
-        int denom = rnd(8), w0 = rndr(-128, 127), w1 = rndr(-128, 127), o0 = rndr(-128, 127), o1 = rndr(-128, 127);
+        /* explicit weights: luma_weight = 2^denom + delta, delta and the offsets in [-128, 127] (hevc.c:251); the limits a quarter of the time */
+        int denom = rnd(8), w0 = (1 << denom) + (rnd(4) ? rndr(-128, 127) : rnd(2) ? -128 : 127), w1 = (1 << denom) + (rnd(4) ? rndr(-128, 127) : rnd(2) ? -128 : 127);
+        int o0 = rnd(4) ? rndr(-128, 127) : rnd(2) ? -128 : 127, o1 = rnd(4) ? rndr(-128, 127) : rnd(2) ? -128 : 127;
         uint16_t *od = plane_to_u16(&dst), *or0 = plane_to_u16(&r0), *or1 = plane_to_u16(&r1);
 
         /* reference: mimic hevc.c:1641-1790 (pointer + optional edge emulation + table call) */
@@ -187,6 +223,7 @@ static void test_mc(HEVCDSPContext *d, VideoDSPContext *vd, int bd, int trials)
         m.sx0 = sx[0]; m.sy0 = sy[0]; m.sx1 = sx[1]; m.sy1 = sy[1]; m.frac0 = mx0 | my0 << 4; m.frac1 = mx1 | my1 << 4;
         m.w0 = w0; m.w1 = w1; m.o0 = o0; m.o1 = o1; m.denom = denom;
         orc_mc_rec(&m, od, PW, or0, or1, PW, PH, bd);
+        if (bi && !chroma && mx0 == 2 && my0 == 2) g_wraps += qpel22_exceeds_int16(&r0, sx[0], sy[0], w, h, bd);
         CHECK(!plane_cmp(&dst, od), "mc bd%d chroma%d %dx%d bi%d w%d frac %d,%d %d,%d edge%d src %d,%d", bd, chroma, w, h, bi, weighted, mx0, my0, mx1, my1, edge, sx[0], sy[0]);
         free(od); free(or0); free(or1); free(emu[0]); free(emu[1]);
         plane_free(&r0); plane_free(&r1); plane_free(&dst);
@@ -344,7 +381,10 @@ int main(int argc, char **argv)
         ff_hevc_dsp_init(&d, bd); ff_videodsp_init(&vd, bd);
         int f0 = g_fail;
         test_transforms(&d, bd, trials * 4);     printf("bd%-2d transforms  fails %d\n", bd, g_fail - f0); f0 = g_fail;
-        test_mc(&d, &vd, bd, trials);             printf("bd%-2d mc          fails %d\n", bd, g_fail - f0); f0 = g_fail;
+        const int w0 = g_wraps;
+        test_mc(&d, &vd, bd, trials);             printf("bd%-2d mc          fails %d, blocks whose list 0 wrapped in int16 %d\n", bd, g_fail - f0, g_wraps - w0);
+        CHECK(g_wraps > w0, "bd%d: no bi-predicted block took list 0 beyond int16", bd);
+        f0 = g_fail;
         for (int cfi = 1; cfi <= 3; cfi++) test_intra(bd, trials, cfi);
         printf("bd%-2d intra       fails %d\n", bd, g_fail - f0); f0 = g_fail;
         test_deblock(&d, bd, trials * 2);         printf("bd%-2d deblock     fails %d\n", bd, g_fail - f0); f0 = g_fail;

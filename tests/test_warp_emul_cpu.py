@@ -56,6 +56,8 @@ def test_emulated_library_has_the_product_abi():
 PARITY = ["test_weighted_prediction_and_sao_restore", "test_constrained_intra_pred", "test_sao_restore_of_bypass_pus", "test_intra_only_small_blocks",
           "test_stages_individually", "test_far_out_of_picture_motion", "test_pcm_and_exotic_transform_paths", "test_malformed_blobs_are_rejected_not_executed",
           "test_malformed_inter_records_are_rejected_on_the_device", "test_empty_work_list_and_smallest_pictures"]
+# tests/test_mc_limits_gpu.py: inter prediction at the limits of its input space, and block-form lists that leave tiles unwritten
+MC_LIMITS = ["test_mc_block_with_tiles_in_two_buckets", "test_small_tile_region_need_not_be_bucket_ordered", "test_malformed_block_lists_are_rejected_on_the_device"]
 
 
 @needs_emul
@@ -63,6 +65,27 @@ PARITY = ["test_weighted_prediction_and_sao_restore", "test_constrained_intra_pr
 def test_gpu_parity_test_on_the_emulated_kernels(emulated, name):
     import test_parity_gpu
     getattr(test_parity_gpu, name)()
+
+
+@needs_emul
+@pytest.mark.parametrize("name", MC_LIMITS)
+def test_mc_limits_on_the_emulated_kernels(emulated, name):
+    import test_mc_limits_gpu
+    getattr(test_mc_limits_gpu, name)()
+
+
+@needs_emul
+@pytest.mark.parametrize("cfi,bd", [(1, 8), (1, 10), (1, 12), (2, 10), (3, 8)])
+def test_mc_limits_sweep_on_the_emulated_kernels(emulated, cfi, bd):
+    import test_mc_limits_gpu
+    test_mc_limits_gpu.test_mc_sweep(cfi, bd)
+
+
+@needs_emul
+@pytest.mark.parametrize("w,h,cfi,bd", [(16, 16, 1, 8), (72, 40, 1, 10), (24, 40, 2, 10), (40, 24, 3, 8)])
+def test_mc_limits_small_pictures_on_the_emulated_kernels(emulated, w, h, cfi, bd):
+    import test_mc_limits_gpu
+    test_mc_limits_gpu.test_mc_sweep_small_pictures(w, h, cfi, bd)
 
 
 @needs_emul
@@ -134,7 +157,10 @@ def test_address_sanitizer_sees_no_out_of_bounds_access_in_the_kernels():
             "T.run_sequence(192, 128, 2, 8, seeds=[66, 67], cip=True, p_intra=0.5)\n"
             "T.test_far_out_of_picture_motion()\n"
             "T.test_malformed_blobs_are_rejected_not_executed()\n"
-            "T.test_malformed_inter_records_are_rejected_on_the_device()\n" % (ROOT, HERE, asan_lib))
+            "T.test_malformed_inter_records_are_rejected_on_the_device()\n"
+            "import test_mc_limits_gpu as M\n"
+            "M.test_malformed_block_lists_are_rejected_on_the_device()\n"
+            "M.test_mc_sweep(1, 10)\n" % (ROOT, HERE, asan_lib))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1800,
                        env=dict(os.environ, LD_PRELOAD=rt, ASAN_OPTIONS="detect_leaks=0:detect_stack_use_after_return=0"))
     assert r.returncode == 0 and "ERROR: AddressSanitizer" not in r.stderr, r.stderr[-4000:]
