@@ -143,6 +143,9 @@ enum {
 };
 #define B200_TUF_RDPCM      1u /* followed by hevcdsp.transform_rdpcm()      hevc_cabac.c:1873,1892 */
 #define B200_TUF_RDPCM_VERT 2u /* rdpcm mode 1 (running sum down the columns)                      */
+/* Either rdpcm flag is legal on B200_TU_SKIP and B200_TU_BYPASS only, as in the reference.  The device applies the vertical
+   running sum between its two transform stages and would apply it to PCM samples, so any other kind with an rdpcm flag is
+   rejected (k_validate; b200_rec_tu returns B200_EINVAL). */
 #define B200_TUF_PARK       4u /* intra TU: leave the residual in the pool (K3 adds it after prediction) */
 
 typedef struct B200TuRec {       /* 16 bytes */

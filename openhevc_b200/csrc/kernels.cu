@@ -87,7 +87,8 @@ __global__ void __launch_bounds__(256) k_validate(ValidateArgs a, uint32_t *gate
         const unsigned long long need = (unsigned long long)t.coeff_off + ((t.flags & B200_TUF_PARK) ? 2 : 0) + (t.nnz == B200_TU_DENSE ? n * n : 2ull * t.nnz);
         if (t.plane > 2 || (1 << t.log2) != n || t.x + n > pw || t.y + n > ph || need > a.ncoef ||
             (t.nnz != B200_TU_DENSE && (int)t.nnz > n * n) || (t.kind == B200_TU_PCM && t.nnz != B200_TU_DENSE) ||
-            t.kind > B200_TU_PCM || (t.kind == B200_TU_DST && n != 4))
+            t.kind > B200_TU_PCM || (t.kind == B200_TU_DST && n != 4) ||
+            ((t.flags & (B200_TUF_RDPCM | B200_TUF_RDPCM_VERT)) && t.kind != B200_TU_SKIP && t.kind != B200_TU_BYPASS))
             bad |= 1u << s;
     }
     if (i < a.sec[B200_SEC_INTRA].count) {

@@ -216,6 +216,8 @@ static int rec_tu_impl(B200Rec *r, int plane, int x, int y, int log2, int kind, 
     const int n = 1 << log2;
     if (x < 0 || y < 0 || x + n > r->pw[plane] || y + n > r->ph[plane]) return B200_EINVAL;
     if (kind == B200_TU_DST && log2 != 2) return B200_EINVAL;
+    // rdpcm follows transform skip or bypass only (hevc_cabac.c:1873,1892); the device would apply it in another order
+    if ((flags & (B200_TUF_RDPCM | B200_TUF_RDPCM_VERT)) && kind != B200_TU_SKIP && kind != B200_TU_BYPASS) return B200_EINVAL;
     // residual of an intra TU: park it, the intra kernel adds it right after predicting the block
     const int li = r->last_intra[plane];
     bool link = false;

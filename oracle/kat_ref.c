@@ -38,7 +38,7 @@ static uint64_t rnd64(void) { uint64_t z = (g_seed += 0x9E3779B97F4A7C15ULL); z 
 static int rnd(int n) { return (int)(rnd64() % (uint64_t)n); }
 static int rndr(int lo, int hi) { return lo + rnd(hi - lo + 1); }
 
-static int g_fail, g_checks, g_wraps;
+static int g_fail, g_checks, g_wraps, g_strong, g_strong_edge[2], g_bclip[2];
 #define CHECK(cond, ...) do { g_checks++; if (!(cond)) { if (g_fail < 20) { fprintf(stderr, "MISMATCH: " __VA_ARGS__); fprintf(stderr, "\n"); } g_fail++; } } while (0)
 
 /* native-format plane (uint8 for 8 bit, uint16 above) <-> oracle uint16 plane */
@@ -92,14 +92,29 @@ static int plane_cmp(const Plane *p, const uint16_t *o)
 }
 
 /* ---------------------------------------------------------------- transforms */
+/* sign of T[j][r], weight of input j in output r of the N-point inverse DCT (HEVC core transform), or of the inverse DST-VII */
+static int basis_sign(int dst, int n, int j, int r)
+{
+    static const int8_t D[4][4] = { { 29, 55, 74, 84 }, { 74, 74, 0, -74 }, { 84, -29, -74, 55 }, { 55, -84, 74, -29 } };
+    if (dst) return D[j][r] >= 0 ? 1 : -1;
+    const int m = ((2 * r + 1) * j * (32 / n)) & 127;           /* T32[j * 32 / n][r] = +-|cos(m * pi / 64)| */
+    return (m <= 32 || m >= 96) ? 1 : -1;
+}
 static void test_transforms(HEVCDSPContext *d, int bd, int trials)
 {
     for (int t = 0; t < trials; t++) {
         int log2 = rndr(2, 5), n = 1 << log2, n2 = n * n;
         DECLARE_ALIGNED(32, int16_t, a[1024]); DECLARE_ALIGNED(32, int16_t, b[1024]);
-        int style = rnd(4);
+        int style = rnd(5), which = rnd(8);
         memset(a, 0, sizeof(a));
-        for (int i = 0; i < n2; i++) {
+        if (style == 4) {   /* basis sign pattern: the sign of coefficient (j, i) is that of basis entry j of output row r times entry i of
+                             * output column c, so every first-stage sum of row r is as large as int32 input allows (far beyond int16) */
+            const int m = which == 5 ? 4 : n, r = rnd(m), c = rnd(m), big = rnd(2) ? 32767 : -32768;
+            for (int j = 0; j < m; j++)
+                for (int i = 0; i < m; i++)
+                    a[j * m + i] = (int16_t)((basis_sign(which == 5, m, j, r) * basis_sign(which == 5, m, i, c) > 0) ? big : (big < 0 ? 32767 : -32768));
+        }
+        for (int i = 0; i < n2 && style != 4; i++) {
             int v = 0;
             if (style == 0) v = rndr(-32768, 32767);                         /* dense, full range */
             else if (style == 1) v = rnd(4) ? 0 : rndr(-2000, 2000);         /* sparse moderate */
@@ -108,7 +123,6 @@ static void test_transforms(HEVCDSPContext *d, int bd, int trials)
             a[i] = (int16_t)v;
         }
         memcpy(b, a, sizeof(a));
-        int which = rnd(8);
         if (which <= 3) {
             int col_limit = rnd(3) ? rndr(1, 2 * n + 4) : n;
             d->idct[log2 - 2](a, col_limit); orc_idct(b, log2, col_limit, bd);
@@ -231,6 +245,59 @@ static void test_mc(HEVCDSPContext *d, VideoDSPContext *vd, int bd, int trials)
 }
 
 /* ---------------------------------------------------------------- intra prediction */
+/* the top row (from the corner to index 2n - 1) and the left column of an n x n block at (x, y) of plane p, where they exist */
+static void fill_neighbours(Plane *p, int x, int y, int n, int content)
+{
+    const int maxv = (1 << p->bd) - 1, thr = 1 << (p->bd - 5);
+    int top[65], left[65];                                   /* [k] = index k - 1 */
+    if (content == 1) {
+        const int st = rnd(maxv / 70 + 1), sl = rnd(maxv / 70 + 1), base = rndr(thr + 1, maxv - 65 * FFMAX(st, sl) - thr - 1);
+        for (int k = 0; k <= 2 * n; k++) { top[k] = base + st * k; left[k] = base + sl * k; }
+        const int d = (int[3]){ 0, thr - 1, thr }[rnd(3)];
+        int *side = rnd(2) ? top : left;
+        side[2 * n] += side[2 * n] + d <= maxv ? d : -d;
+    } else if (content == 2) {
+        const int kind = rnd(3);
+        for (int k = 0; k <= 2 * n; k++) top[k] = left[k] = kind == 0 ? 0 : kind == 1 ? maxv : (k & 1) * maxv;
+    } else {
+        const int hi = rnd(2);
+        for (int k = 0; k <= 2 * n; k++) top[k] = left[k] = (k == 0) == hi ? 0 : maxv;
+    }
+    if (y > 0) for (int k = 0; k <= 2 * n && x - 1 + k < p->w; k++) if (x - 1 + k >= 0) plane_put(p, x - 1 + k, y - 1, top[k]);
+    if (x > 0) for (int k = 0; k <= 2 * n && y - 1 + k < p->h; k++) if (y - 1 + k >= 0) plane_put(p, x - 1, y - 1 + k, left[k]);
+}
+
+/* what the block's prediction must go through, restated where the up-left, up and left neighbours exist (the reference
+ * arrays are then the picture's samples, with the unavailable or out-of-picture part of the up-right / bottom-left halves
+ * replaced by the last sample before it): strong smoothing decisions (and blocks one step either side of the threshold),
+ * and the mode-26 / mode-10 boundary filters clipped at 0 and at max */
+static void count_intra_limits(const B200IntraRec *r, const uint16_t *o, int pw, int ph, int bd)
+{
+    const int need = B200_INF_UP_LEFT | B200_INF_UP | B200_INF_LEFT;
+    if ((r->flags & need) != need) return;
+    const int n = 1 << r->log2, x = r->x, y = r->y, maxv = (1 << bd) - 1, thr = 1 << (bd - 5);
+    int tb[65], lb[65], *top = tb + 1, *left = lb + 1;
+    top[-1] = left[-1] = o[(y - 1) * pw + x - 1];
+    for (int i = 0; i < n; i++) { top[i] = o[(y - 1) * pw + x + i]; left[i] = o[(y + i) * pw + x - 1]; }
+    for (int i = 0; i < n; i++) {
+        top[n + i] = (r->flags & B200_INF_UP_RIGHT) ? o[(y - 1) * pw + x + n + FFMIN(i, r->top_right_size - 1)] : top[n - 1];
+        left[n + i] = (r->flags & B200_INF_BOTTOM_LEFT) ? o[(y + n + FFMIN(i, r->bottom_left_size - 1)) * pw + x - 1] : left[n - 1];
+    }
+    (void)ph;
+    const int mode = r->mode;
+    if (r->plane == 0 && n < 32 && (mode == 10 || mode == 26))
+        for (int i = 0; i < n; i++) {
+            const int v = mode == 26 ? top[0] + ((left[i] - left[-1]) >> 1) : left[0] + ((top[i] - top[-1]) >> 1);
+            if (v < 0) { g_bclip[0]++; break; }
+            if (v > maxv) { g_bclip[1]++; break; }
+        }
+    if (r->plane == 0 && r->log2 == 5 && (r->flags & B200_INF_FILTER) && (r->flags & B200_INF_STRONG) && mode != 1 && mode != 10 && mode != 26) {
+        const int d = FFMAX(abs(top[-1] + top[63] - 2 * top[31]), abs(left[-1] + left[63] - 2 * left[31]));
+        g_strong += d < thr;
+        g_strong_edge[0] += d == thr - 1;
+        g_strong_edge[1] += d == thr;
+    }
+}
 static void test_intra(int bd, int trials, int cfi)
 {
     /* a genuine (minimal) decoder context: intra_pred reads sps/pps/frame/HEVClc, hevcpred_template.c:30-110 */
@@ -258,6 +325,12 @@ static void test_intra(int bd, int trials, int cfi)
         sps->sps_strong_intra_smoothing_enable_flag = rnd(2);
         sps->spsRext.intra_smoothing_disabled_flag = rnd(8) == 0;
         int c_idx = rnd(3), log2 = rndr(2, 5), n = 1 << log2;
+        /* neighbour content at the limits: 1 linear ramps, with the second difference at index 31 of one side 0, thr - 1 or
+         * thr (the strong-smoothing test, hevcpred_template.c:296-300); 2 all 0, all max or 0 / max alternating; 3 corner
+         * and top / left at opposite ends (the mode-10 / mode-26 boundary filters past 0 or max) */
+        const int content = rnd(3) ? 0 : 1 + rnd(3);
+        if (content == 1 && rnd(2)) c_idx = 0, log2 = 5, n = 32;
+        if (content == 3 && rnd(2)) c_idx = 0, log2 = rndr(2, 4), n = 1 << log2;
         if (c_idx && cfi != 3 && log2 == 5 && rnd(2)) log2 = 4, n = 16;
         int hs = sps->hshift[c_idx], vs = sps->vshift[c_idx];
         int nl_h = n << hs, nl_v = n << vs;               /* size in luma units */
@@ -266,7 +339,8 @@ static void test_intra(int bd, int trials, int cfi)
         if (rnd(3) == 0) x0 = rnd(2) ? 0 : W - nl_h;
         if (rnd(3) == 0) y0 = rnd(2) ? 0 : H - nl_v;
         int mode = rnd(4) == 0 ? rnd(2) : rndr(2, 34);
-        if (rnd(6) == 0) mode = rnd(2) ? 10 : 26;
+        if (rnd(6) == 0 || content == 3) mode = rnd(2) ? 10 : 26;
+        if (content) fill_neighbours(&pl[c_idx], x0 >> hs, y0 >> vs, n, content);
         lc->tu.intra_pred_mode = lc->tu.intra_pred_mode_c = mode;
         /* CTB neighbourhood flags as hls_decode_neighbour would set them for a single slice / tile (hevc.c:2590-2660) */
         int xc = x0 >> 6, yc = y0 >> 6;
@@ -293,6 +367,7 @@ static void test_intra(int bd, int trials, int cfi)
         r.bottom_left_size = (FFMIN(y0 + 2 * nl_v, H) - (y0 + nl_v)) >> vs;
         r.top_right_size = (FFMIN(x0 + 2 * nl_h, W) - (x0 + nl_h)) >> hs;
         r.resid_off = B200_NO_RESID;
+        count_intra_limits(&r, op[c_idx], pl[c_idx].w, pl[c_idx].h, bd);
         orc_intra_rec(&r, op[c_idx], pl[c_idx].w, bd);
         CHECK(!plane_cmp(&pl[c_idx], op[c_idx]), "intra bd%d cfi%d c%d n%d mode%d at %d,%d flags %x", bd, cfi, c_idx, n, mode, x0, y0, r.flags);
         for (int c = 0; c < 3; c++) { free(op[c]); plane_free(&pl[c]); }
@@ -385,8 +460,13 @@ int main(int argc, char **argv)
         test_mc(&d, &vd, bd, trials);             printf("bd%-2d mc          fails %d, blocks whose list 0 wrapped in int16 %d\n", bd, g_fail - f0, g_wraps - w0);
         CHECK(g_wraps > w0, "bd%d: no bi-predicted block took list 0 beyond int16", bd);
         f0 = g_fail;
+        const int s0 = g_strong, e0 = g_strong_edge[0], e1 = g_strong_edge[1], c0 = g_bclip[0], c1 = g_bclip[1];
         for (int cfi = 1; cfi <= 3; cfi++) test_intra(bd, trials, cfi);
-        printf("bd%-2d intra       fails %d\n", bd, g_fail - f0); f0 = g_fail;
+        printf("bd%-2d intra       fails %d, strong smoothing %d (at threshold - 1: %d, at threshold: %d), boundary filter clipped at 0: %d, at max: %d\n",
+               bd, g_fail - f0, g_strong - s0, g_strong_edge[0] - e0, g_strong_edge[1] - e1, g_bclip[0] - c0, g_bclip[1] - c1);
+        CHECK(g_strong > s0, "bd%d: no 32x32 luma block took strong smoothing", bd);
+        CHECK(g_bclip[0] > c0 && g_bclip[1] > c1, "bd%d: the mode-10 / mode-26 boundary filters were not clipped at both ends", bd);
+        f0 = g_fail;
         test_deblock(&d, bd, trials * 2);         printf("bd%-2d deblock     fails %d\n", bd, g_fail - f0); f0 = g_fail;
         test_sao(&d, bd, trials);                 printf("bd%-2d sao         fails %d\n", bd, g_fail - f0);
     }

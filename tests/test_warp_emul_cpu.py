@@ -89,6 +89,39 @@ def test_mc_limits_small_pictures_on_the_emulated_kernels(emulated, w, h, cfi, b
 
 
 @needs_emul
+@pytest.mark.parametrize("cfi,bd", [(1, 8), (1, 10), (1, 12), (2, 10), (3, 8)])
+def test_residual_limits_sweep_on_the_emulated_kernels(emulated, cfi, bd):
+    """tests/test_residual_intra_limits_gpu.py: the residual sweep with impulses at every 37th coefficient position (the
+    GPU run takes every position)"""
+    import test_residual_intra_limits_gpu as T
+    T.run_residual_sweep((256, 128, cfi, bd), seed=10 * cfi + bd, impulse_step=37)
+
+
+@needs_emul
+@pytest.mark.parametrize("cfi,bd", [(1, 8), (1, 10), (1, 12), (2, 10), (3, 8)])
+def test_intra_limits_sweep_on_the_emulated_kernels(emulated, cfi, bd):
+    import test_residual_intra_limits_gpu as T
+    T.test_intra_sweep(cfi, bd)
+
+
+@needs_emul
+@pytest.mark.parametrize("name", ["test_residual_sweep_small_pictures", "test_intra_sweep_small_pictures", "test_intra_dense_zorder"])
+def test_residual_intra_limits_small_and_dense_on_the_emulated_kernels(emulated, name):
+    """one of the three geometries the GPU run takes for each (the residual sweep with impulses at every 37th position)"""
+    import test_residual_intra_limits_gpu as T
+    if name == "test_residual_sweep_small_pictures":
+        T.run_residual_sweep((72, 40, 1, 10), seed=1, impulse_step=37)
+    else:
+        getattr(T, name)(*{"test_intra_sweep_small_pictures": (24, 40, 2, 12), "test_intra_dense_zorder": (72, 40, 2, 10)}[name])
+
+
+@needs_emul
+def test_rdpcm_rejection_on_the_emulated_kernels(emulated):
+    import test_residual_intra_limits_gpu as T
+    T.test_rdpcm_on_transformed_or_pcm_blocks_is_rejected()
+
+
+@needs_emul
 @pytest.mark.parametrize("w,h,cfi,bd", [(256, 128, 1, 8), (256, 128, 1, 10), (192, 128, 2, 10), (192, 128, 3, 8), (320, 192, 1, 12)])
 def test_sequence_all_stages_on_the_emulated_kernels(emulated, w, h, cfi, bd):
     import test_parity_gpu
@@ -136,6 +169,18 @@ def test_switch_variants_on_the_emulated_kernels(env):
 
 
 @needs_emul
+def test_intra_limits_sweep_in_reverse_lane_order():
+    """the intra sweep with the emulator running the lanes between two collectives in reverse order"""
+    code = ("import sys; sys.path[:0] = [%r, %r]\n"
+            "from openhevc_b200 import _lib; _lib.LIB_PATH = %r\n"
+            "import test_residual_intra_limits_gpu as R\n"
+            "R.test_intra_sweep(1, 10)\n"
+            "R.test_intra_dense_zorder(72, 40, 2, 10)\n" % (ROOT, HERE, EMUL))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, env=dict(os.environ, B200_EMUL_ORDER="reverse"))
+    assert r.returncode == 0, r.stderr[-3000:]
+
+
+@needs_emul
 def test_smoke_on_the_emulated_kernels(emulated, capsys):
     import __graft_entry__
     __graft_entry__.smoke()
@@ -160,7 +205,10 @@ def test_address_sanitizer_sees_no_out_of_bounds_access_in_the_kernels():
             "T.test_malformed_inter_records_are_rejected_on_the_device()\n"
             "import test_mc_limits_gpu as M\n"
             "M.test_malformed_block_lists_are_rejected_on_the_device()\n"
-            "M.test_mc_sweep(1, 10)\n" % (ROOT, HERE, asan_lib))
+            "M.test_mc_sweep(1, 10)\n"
+            "import test_residual_intra_limits_gpu as R\n"
+            "R.test_rdpcm_on_transformed_or_pcm_blocks_is_rejected()\n"
+            "R.test_intra_sweep(1, 12)\n" % (ROOT, HERE, asan_lib))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1800,
                        env=dict(os.environ, LD_PRELOAD=rt, ASAN_OPTIONS="detect_leaks=0:detect_stack_use_after_return=0"))
     assert r.returncode == 0 and "ERROR: AddressSanitizer" not in r.stderr, r.stderr[-4000:]
