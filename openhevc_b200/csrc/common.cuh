@@ -16,8 +16,8 @@ struct RefTable {
     uint64_t w[2];      // B200BlobHeader.ref_slot[16] packed little-endian (possibly overridden at execute time)
 };
 
-// HD: code that is also compiled for the host so that tests/ can run the very same per-thread code on the CPU
-// (csrc/emul.cu, test infrastructure; the product library never executes it on the host)
+// HD: code that is also compiled for the host (with plain-C versions of the 16x2 instructions below) so that the CPU suite's
+// warp emulator (tests/emul/warp/, test infrastructure) runs the very same source; the product never executes it on the host
 #define HD __host__ __device__ __forceinline__
 HD int clip3i(int v, int lo, int hi) { return v < lo ? lo : v > hi ? hi : v; }
 HD int clip16i(int v) { return v < -32768 ? -32768 : v > 32767 ? 32767 : v; }

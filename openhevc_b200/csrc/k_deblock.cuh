@@ -1,6 +1,6 @@
 // k_deblock.cuh — per-thread code of the deblocking stage (K4).  Host + device: kernels.cu wraps the four phases in the
-// __global__ kernel (with __syncthreads() between them); tests/emul/kernel_emul.cu (test infrastructure) runs the same
-// functions thread by thread on the CPU.
+// __global__ kernel (with __syncthreads() between them); the CPU suite's warp emulator (tests/emul/warp/) runs that
+// kernel, these functions included, on the host.
 //
 // hevc_{h,v}_loop_filter_{luma,chroma}, hevcdsp_template.c:1629-1787.  Both directions in ONE pass: tiles are offset
 // by (-4,-4) from the 8x8 edge grid, so every sample an edge reads or writes (<= 4 on either side) belongs to exactly

@@ -1,8 +1,8 @@
 // k_intra_cip.cuh — constrained_intra_pred for the intra stage (K3): hevcpred_template.c:116-163 (which neighbours
 // stay candidates) and :185-249 (samples of inter-coded neighbours are replaced by the nearest intra-coded ones).
 // Host + device: k_intra runs both functions on lane 0 of the warp that owns the TU (the rules are a sequential scan
-// over at most 129 samples, and constrained_intra_pred streams are rare); tests/emul/kernel_emul.cu runs them on the CPU
-// against the oracle.
+// over at most 129 samples, and constrained_intra_pred streams are rare); the CPU suite's warp emulator (tests/emul/warp/)
+// runs k_intra, these functions included, on the host against the oracle.
 //
 // Arrays: top[-1 .. 2n-1], left[-1 .. 2n-1] as plain int pointers (index -1 = the corner), already holding the
 // candidate samples (and the reference's memset pattern everywhere else, :159-161) when cip_substitute() is called.

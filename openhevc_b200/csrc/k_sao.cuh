@@ -1,6 +1,6 @@
 // k_sao.cuh — per-thread code of the SAO stage (K5).  Host + device: kernels.cu wraps sao_thread() in the __global__
-// kernel; tests/emul/kernel_emul.cu (test infrastructure) runs the same function thread by thread on the CPU so that
-// the packed arithmetic is checked against the oracle before it ever reaches a GPU.
+// kernel; the CPU suite's warp emulator (tests/emul/warp/) compiles kernels.cu for the host, so the packed arithmetic is
+// checked against the oracle, through the product's own launcher, before it ever reaches a GPU.
 #pragma once
 #include "common.cuh"
 

@@ -365,7 +365,6 @@ static const int8_t k_intra_angle[33] = { 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5
 static const int16_t k_inv_angle[15] = { -4096, -1638, -910, -630, -482, -390, -315, -256, -315, -390, -482, -630, -910, -1638, -4096 };
 
 static void orc_intra_rec_cip(const B200IntraRec *r, pix_t *plane, int stride, int bd, const OrcCip *cip);
-static int *g_cap_top, *g_cap_left, *g_cap_flags;      /* test hook, see orc_debug_cip_refs() */
 void orc_intra_rec(const B200IntraRec *r, pix_t *plane, int stride, int bd) { orc_intra_rec_cip(r, plane, stride, bd, NULL); }
 
 static void orc_intra_rec_cip(const B200IntraRec *r, pix_t *plane, int stride, int bd, const OrcCip *cip)
@@ -398,12 +397,6 @@ static void orc_intra_rec_cip(const B200IntraRec *r, pix_t *plane, int stride, i
         for (; i < n; i++) left[n + i] = src[(n + r->bottom_left_size - 1) * stride - 1];
     }
     if (cip) orc_cip_substitute(r, cip, left, top, up_left, up, up_right, lft, bottom_left);
-    if (g_cap_top) {                 /* orc_debug_cip_refs(): hand out the arrays as they stand here, predict nothing */
-        for (i = -1; i < 64; i++) { g_cap_top[i + 1] = top[i]; g_cap_left[i + 1] = left[i]; }
-        *g_cap_flags = (up_left ? B200_INF_UP_LEFT : 0) | (up ? B200_INF_UP : 0) | (up_right ? B200_INF_UP_RIGHT : 0) |
-                       (lft ? B200_INF_LEFT : 0) | (bottom_left ? B200_INF_BOTTOM_LEFT : 0);
-        return;
-    }
     /* substitution chain (:250-286) */
     if (!bottom_left) {
         if (lft) { for (i = 0; i < n; i++) left[n + i] = left[n - 1]; }
@@ -1036,24 +1029,5 @@ int orc_execute_blob(const uint8_t *blob, uint16_t **planes, int n_slots)
             free(copy);
         }
     }
-    return 0;
-}
-
-/* Test hook for tests/test_kernel_emul_cpu.py: the reference arrays of intra record `rec_index` of a constrained_intra_pred
- * blob after the CIP rules (:116-249), before the ordinary substitution -- neighbours are read from `planes` (the
- * picture of the current slot) as they are.  top65 / left65: index 0 holds [-1].  Not thread safe. */
-int orc_debug_cip_refs(const uint8_t *blob, uint16_t **planes, int rec_index, int *top65, int *left65, int *flags_out)
-{
-    const B200BlobHeader *h = (const B200BlobHeader *)blob;
-    if (h->magic != B200_BLOB_MAGIC || !(h->flags & B200_FRAME_CIP) || h->cip.count < 4 || rec_index < 0 || (uint32_t)rec_index >= h->sec[B200_SEC_INTRA].count) return -1;
-    const uint32_t *cw = (const uint32_t *)(blob + h->cip.off);
-    const B200IntraRec *r = (const B200IntraRec *)(blob + h->sec[B200_SEC_INTRA].off) + rec_index;
-    const int cfi = h->chroma_format_idc, p = r->plane;
-    OrcCip cip = { (int)cw[0], (int)cw[1], (int)cw[2], cw + 4, p && cfi != 3, p && cfi == 1, h->width, h->height };
-    int pw, ph;
-    b200_plane_dims(h->width, h->height, cfi, p, &pw, &ph);
-    g_cap_top = top65; g_cap_left = left65; g_cap_flags = flags_out;
-    orc_intra_rec_cip(r, planes[p], pw, h->bit_depth, &cip);
-    g_cap_top = g_cap_left = g_cap_flags = NULL;
     return 0;
 }

@@ -9,6 +9,7 @@ whole prediction blocks that the device cuts into tiles (k_mc_expand; recorded t
 must equal the CPU oracle, and where the reference's own tables are built (oracle/_ref/libreplay_ref.so) the oracle must equal
 them as well.  Destination rectangles within a picture never overlap, so the order in which tiles run cannot matter."""
 import ctypes as C
+import os
 
 import numpy as np
 import pytest
@@ -16,6 +17,7 @@ import pytest
 import oracle_lib
 from openhevc_b200 import FrameEngine, B200Error, _lib
 from openhevc_b200 import worklist as W
+from openhevc_b200.synth import FrameSynth, smooth_frame
 
 pytestmark = pytest.mark.gpu
 
@@ -245,6 +247,27 @@ def check_picture(eng, geom, recs, dpb, what, reference_tables=True, blobs=None)
         assert_same(eng.decode(blob), want, f"{what} {form}")
 
 
+def padded_engine(geom, n_slots, **kw):
+    """a FrameEngine on a caller-owned DPB (ext_frame_mem) whose every byte starts as 0x5a: garbage in the row padding of
+    each slot, which no kernel may read.  A torch CUDA tensor on the device; the emulated library's device memory is host
+    memory, so there a numpy buffer."""
+    width, height, cfi, bd = geom
+    cfg = _lib.B200Config(0, width, height, cfi, bd, 6, n_slots, 2, 0, None, 0)
+    nbytes = int(_lib.load().b200_dpb_bytes(C.byref(cfg)))
+    if "_emul" in os.path.basename(_lib.LIB_PATH):
+        raw = np.full(nbytes + 256, 0x5a, np.uint8)
+        mem = raw[-raw.ctypes.data % 256:][:nbytes]                   # ext_frame_mem must be 256-byte aligned
+        ptr = mem.ctypes.data
+    else:
+        import torch
+        mem = torch.full((nbytes,), 0x5a, dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        ptr = mem.data_ptr()
+    eng = FrameEngine(*geom, n_slots=n_slots, ext_frame_mem=ptr, ext_frame_bytes=nbytes, **kw)
+    eng.dpb_mem = mem                                                  # the engine does not own it: keep it alive as long
+    return eng
+
+
 def run_sweep(geom, contents, rects_per_picture, seed, wrap_guard=True):
     eng = FrameEngine(*geom, n_slots=3)
     k, signed = [0, 0], []
@@ -280,6 +303,38 @@ def test_mc_sweep_small_pictures(w, h, cfi, bd):
     """pictures of one partial CTB: every block is near a border, many windows hang over two of them"""
     pics = pack([s for s in luma_shapes() if s[0] <= w and s[1] <= h], w, h)
     run_sweep((w, h, cfi, bd), ("sign", "noise"), pics, seed=w + h + bd, wrap_guard=False)     # windows too large to lie inside
+
+
+MC_CASES = [  # w, h, cfi, bd, FrameSynth arguments
+    (256, 128, 1, 8, {}),
+    (256, 128, 1, 10, dict(weighted=True)),
+    (320, 192, 1, 10, dict(max_mv=150)),               # windows far outside the picture: clamped loads
+    (192, 128, 2, 10, {}),
+    (192, 128, 3, 8, dict(weighted=True)),
+    (320, 192, 1, 12, dict(split_bias=2.5)),           # many small blocks
+    (256, 192, 1, 10, dict(split_bias=0.3, bi_frac=0.2)),
+]
+
+
+@pytest.mark.late
+@pytest.mark.parametrize("w,h,cfi,bd,kw", MC_CASES)
+def test_mc_synthetic_pictures(w, h, cfi, bd, kw):
+    """pure inter pictures of the synthetic quadtrees: every PU shape they produce, all 16 / 64 phases, uni / bi / weighted,
+    windows over the picture border, tiles of one warp and of 8-lane groups; garbage in the row padding of the references and
+    of the current picture"""
+    eng = padded_engine((w, h, cfi, bd), n_slots=3)
+    try:
+        for seed in range(2):
+            blob, st = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=800 + 10 * seed + bd + cfi, refs=[1, 2], cur_slot=0, p_intra=0.0, coded_frac=0.0,
+                                  deblock=False, sao=False, **kw).generate()
+            hdr, secs = W.parse_blob(blob)
+            assert len(secs[W.SEC_INTRA]) == 0 and sum(len(secs[k]) for k in (W.SEC_TU4, W.SEC_TU8, W.SEC_TU16, W.SEC_TU32)) == 0
+            dpb = [smooth_frame(w, h, cfi, bd, 300 + k) for k in range(3)]
+            for slot in (1, 2):
+                eng.upload_slot(slot, dpb[slot])
+            assert_same(eng.decode(blob), oracle_lib.execute(blob, dpb), f"seed {seed}")
+    finally:
+        eng.close()
 
 
 def test_mc_block_with_tiles_in_two_buckets():

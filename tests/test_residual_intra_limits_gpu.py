@@ -610,6 +610,54 @@ def test_intra_dense_zorder(w, h, cfi, bd):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# constrained intra prediction in inter pictures
+# ---------------------------------------------------------------------------------------------------------------------
+def all_intra_cip(blob):
+    """the same picture with every min-PU of its constrained_intra_pred bitmap intra"""
+    out = blob.copy()
+    hdr = W.parse_blob(out)[0]
+    off, count = int(hdr["cip"]["off"]), int(hdr["cip"]["count"])
+    out[off + 16:off + 4 * count] = 0xff
+    return out
+
+
+CIP_CASES = [(1, 8, 0.12, 1.0), (1, 10, 0.45, 1.0), (2, 10, 0.3, 2.0), (3, 8, 0.6, 0.5), (1, 12, 0.8, 2.0)]     # cfi, bd, p_intra, split_bias
+
+
+@pytest.mark.late
+@pytest.mark.parametrize("cfi,bd,p_intra,split", CIP_CASES)
+def test_constrained_intra_rules(cfi, bd, p_intra, split):
+    """cip_flags() / cip_substitute() (k_intra_cip.cuh, run by lane 0 of k_intra) against the oracle's restatement of
+    hevcpred_template.c:116-249, for every intra TU of synthetic inter pictures over noise references.  A picture shows only
+    the reference entries its modes read, so each one runs with every intra TU at mode 2, at 18 and at 34, strong smoothing
+    off: between them these read every entry [-1 .. 2N-1] of both arrays, and a wrong entry or flag changes a sample."""
+    from openhevc_b200.synth import FrameSynth
+    w, h = 320, 192
+    geom = (w, h, cfi, bd)
+    blob, st = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=500 + cfi + bd, refs=[1], cur_slot=0, cip=True, p_intra=p_intra, split_bias=split).generate()
+    assert int(W.parse_blob(blob)[0]["flags"]) & W.FRAME_CIP
+    rng = np.random.default_rng(9)
+    dpb = [noise_planes(geom, rng) for _ in range(2)]                 # noise: any mix-up of two samples shows
+    eng = FrameEngine(*geom, n_slots=2)
+    try:
+        eng.upload_slot(1, dpb[1])
+        for mode in (2, 18, 34):
+            b = blob.copy()
+            intra = W.parse_blob(b)[1][W.SEC_INTRA]
+            intra["mode"] = mode
+            intra["flags"] &= 0xff ^ W.INF_STRONG
+            want = oracle_lib.execute(b, dpb)
+            every = oracle_lib.execute(all_intra_cip(b), dpb)
+            changed = sum(bool((want[p][y:y + n, x:x + n] != every[p][y:y + n, x:x + n]).any())
+                          for p, x, y, n in zip(intra["plane"], intra["x"], intra["y"], 1 << intra["log2"].astype(int)))
+            assert changed > 10, "the constrained-intra rule never removed a candidate: the test picture does not exercise it"
+            eng.upload_slot(0, dpb[0])
+            assert_same(eng.decode(b), want, f"{geom} mode {mode}")
+    finally:
+        eng.close()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # rdpcm on blocks the device transforms in another order
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.late

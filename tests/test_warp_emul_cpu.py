@@ -6,7 +6,8 @@ __shfl_*_sync / __syncwarp / vote / __syncthreads, kernel launches, copies and e
 oracle/_ref/libb200hevc_emul.so, has the C ABI of libb200hevc.so.  These tests load it IN PLACE of the CUDA library -- only
 here, the product never does -- and run
 
- * the GPU parity tests (tests/test_parity_gpu.py, same functions, same seeds) against the oracle, and
+ * the GPU parity and limits tests (tests/test_parity_gpu.py, tests/test_*_limits_gpu.py; same functions, same seeds)
+   against the oracle, and
  * the real decoder with the B200 hooks on the committed streams (decode_b200, the emulated library pre-loaded) against
    the MD5s of the unmodified reference decoder,
 
@@ -20,6 +21,9 @@ import sys
 import pytest
 
 import oracle_lib
+import test_loop_filter_limits_gpu as LF
+import test_mc_limits_gpu as MC
+import test_residual_intra_limits_gpu as RI
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -72,6 +76,18 @@ def test_gpu_parity_test_on_the_emulated_kernels(emulated, name):
 def test_mc_limits_on_the_emulated_kernels(emulated, name):
     import test_mc_limits_gpu
     getattr(test_mc_limits_gpu, name)()
+
+
+# the cases of the limits files on synthetic pictures and random grids (K1, K3's constrained-intra rules, K4, K5), every
+# parameter set the GPU run takes
+LIMITS = [(LF, "test_sao_limits", LF.SAO_CASES), (LF, "test_deblock_limits", LF.DBK_CASES), (LF, "test_sao_restore_limits", LF.RESTORE_CASES),
+          (RI, "test_constrained_intra_rules", RI.CIP_CASES), (MC, "test_mc_synthetic_pictures", MC.MC_CASES)]
+
+
+@needs_emul
+@pytest.mark.parametrize("module,name,args", [pytest.param(m, n, a, id=f"{n}-{a}".replace(" ", "")) for m, n, cases in LIMITS for a in cases])
+def test_limits_case_on_the_emulated_kernels(emulated, module, name, args):
+    getattr(module, name)(*args)
 
 
 @needs_emul
