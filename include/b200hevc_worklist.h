@@ -1,5 +1,5 @@
 /*
- * b200hevc_worklist.h — wire format of the per-frame packed work list ("blob v1").
+ * b200hevc_worklist.h — wire format of the per-frame packed work list ("blob v3").
  *
  * The host side of the decoder (openHEVC's CABAC parse / MV / BS derivation, which
  * stays on the CPU) does not execute pixel kernels any more: every call it makes
@@ -32,7 +32,8 @@ enum {
     B200_SEC_TU16,        /* B200TuRec, 16x16                                                      */
     B200_SEC_TU32,        /* B200TuRec, 32x32                                                      */
     B200_SEC_INTRA,       /* B200IntraRec in decode order (intra_pred[] call sites)                */
-    B200_SEC_MC,          /* B200McRec, one per <=256-sample tile of a put_hevc_{q,e}pel* call     */
+    B200_SEC_MC,          /* B200McRec of the put_hevc_{q,e}pel* calls: tiles of <= 256 samples, or whole prediction
+                             blocks that the device cuts into tiles (B200BlobHeader.mc_tile_count says which) */
     B200_SEC_DBK,         /* uint16 edge-parameter grids, layout B200DbkLayout (count = #uint16)   */
     B200_SEC_SAO,         /* B200SaoRec grid [3][ctb_count] (count = 3*ctb_count) or 0 = no SAO    */
     B200_SEC_COUNT
@@ -210,7 +211,7 @@ typedef struct B200IntraRec {    /* 16 bytes */
 
 typedef struct B200McRec {       /* 32 bytes */
     uint16_t x, y;               /* destination top-left sample in its plane */
-    uint8_t  w, h;               /* tile size, w*h <= 256 after recorder splitting, w<=32 */
+    uint8_t  w, h;               /* tile: w*h <= 256, w <= 32; whole block: w, h <= 64 (B200BlobHeader.mc_tile_count) */
     uint8_t  plane;
     uint8_t  flags;              /* B200_MCF_* */
     int16_t  sx0, sy0;           /* integer source position in ref0's plane (may lie outside: samples clamp, videodsp_template.c:26-100) */
@@ -261,10 +262,10 @@ typedef struct B200SaoRec {      /* 16 bytes; grid index = plane * ctb_count + c
 
 #ifdef __cplusplus
 static_assert(sizeof(B200BlobHeader) == 256 && sizeof(B200TuRec) == 16 && sizeof(B200IntraRec) == 16 &&
-              sizeof(B200McRec) == 32 && sizeof(B200SaoRec) == 16, "blob v1 layout");
+              sizeof(B200McRec) == 32 && sizeof(B200SaoRec) == 16, "blob v3 layout");
 #else
 _Static_assert(sizeof(B200BlobHeader) == 256 && sizeof(B200TuRec) == 16 && sizeof(B200IntraRec) == 16 &&
-               sizeof(B200McRec) == 32 && sizeof(B200SaoRec) == 16, "blob v1 layout");
+               sizeof(B200McRec) == 32 && sizeof(B200SaoRec) == 16, "blob v3 layout");
 #endif
 
 /* data of a TU inside the pool; *park_off receives the parked-pool index of PARK TUs */

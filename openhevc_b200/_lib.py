@@ -7,6 +7,14 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_LIB_PATH") or os.path.join(_HERE, "libb200hevc.so")     # (B200_LIB_PATH: tuning builds of the same library, tools/)
 
 
+class B200Error(RuntimeError):
+    """a call of libb200hevc failed; `code` is its B200_E* return value (None where the call returns no code)"""
+
+    def __init__(self, message, code=None):
+        super().__init__(message)
+        self.code = code
+
+
 class B200Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("chroma_format_idc", C.c_int32),
                 ("bit_depth", C.c_int32), ("log2_ctb_size", C.c_int32), ("n_slots", C.c_int32), ("n_arenas", C.c_int32),

@@ -9,13 +9,10 @@ import ctypes as C
 import numpy as np
 
 from . import _lib, device_output
-from .worklist import plane_dims
+from ._lib import B200Error
+from .worklist import header, plane_dims
 
 STAGES = ("mc", "residual", "intra", "deblock", "sao", "total")
-
-
-class B200Error(RuntimeError):
-    pass
 
 
 class PinnedBuffer:
@@ -52,14 +49,14 @@ class FrameEngine:
         h = C.c_void_p()
         rc = self.lib.b200_ctx_create(C.byref(self.cfg), C.byref(h))
         if rc:
-            raise B200Error(f"b200_ctx_create failed ({rc}): {self.lib.b200_last_error(None).decode()}")
+            raise B200Error(f"b200_ctx_create failed ({rc}): {self.lib.b200_last_error(None).decode()}", rc)
         self.h = h
         self._pinned = []
 
     # -- helpers ---------------------------------------------------------------------------------
     def _chk(self, rc):
         if rc:
-            raise B200Error(f"libb200hevc error {rc}: {self.lib.b200_last_error(self.h).decode()}")
+            raise B200Error(f"libb200hevc error {rc}: {self.lib.b200_last_error(self.h).decode()}", rc)
 
     def plane_shape(self, p):
         w, h = plane_dims(self.width, self.height, self.cfi, p)
@@ -151,8 +148,7 @@ class FrameEngine:
         """submit + readback of the picture's DPB slot (blocking): what a caller of the reference's
         libOpenHevcDecode + GetOutput sees for one access unit."""
         self.submit(blob)
-        slot = int(np.asarray(blob[:256]).view(np.uint8)[23])   # header.cur_slot
-        return self.readback(slot, out)
+        return self.readback(int(header(blob)["cur_slot"]), out)
 
     # -- measurement ---------------------------------------------------------------------------------
     def set_profiling(self, on=True):

@@ -1,9 +1,13 @@
-"""numpy mirror of include/b200hevc_worklist.h (blob v3) — builder and parser.
+"""numpy mirror of include/b200hevc_worklist.h (blob v3) — builder, parser and the binding of the C recorder.
 
-Host-side only.  The structured dtypes below are byte-for-byte the C structs; a blob built here
-is what the C recorder (csrc/recorder.cpp) produces for the same table calls.
-"""
+Host-side only.  The structured dtypes below are byte-for-byte the C structs of the same names (tests/test_oracle_cpu.py
+checks them with the C compiler); a blob built here is equivalent to what the C recorder (csrc/recorder.cpp) produces."""
+import ctypes as C
+
 import numpy as np
+
+from . import _lib
+from ._lib import B200Error
 
 MAGIC = 0x4C573242
 VERSION = 3
@@ -16,7 +20,7 @@ INF_UP_LEFT, INF_UP, INF_UP_RIGHT, INF_LEFT, INF_BOTTOM_LEFT, INF_FILTER, INF_ST
 MCF_BI, MCF_WEIGHTED, MCF_CHROMA = 1, 2, 4
 SAO_NONE, SAO_BAND, SAO_EDGE = 0, 1, 2
 NO_RESID = 0xFFFFFFFF
-FRAME_HAS_DEBLOCK, FRAME_HAS_SAO, FRAME_CIP, FRAME_TQB = 1, 2, 4, 8
+FRAME_HAS_DEBLOCK, FRAME_HAS_SAO, FRAME_CIP, FRAME_TQB, FRAME_CCP = 1, 2, 4, 8, 16
 
 section_dt = np.dtype([("off", "<u4"), ("count", "<u4")])
 header_dt = np.dtype([
@@ -25,7 +29,7 @@ header_dt = np.dtype([
     ("log2_ctb_size", "u1"), ("cur_slot", "u1"), ("flags", "<u4"),
     ("sec", section_dt, (SEC_COUNT,)), ("ref_slot", "u1", (16,)), ("n_ref", "u1"), ("pad", "u1", (3,)),
     ("mc_big_count", "<u4"), ("cip", section_dt), ("tqb", section_dt), ("ccp", section_dt), ("dbd", section_dt), ("reserved_section", section_dt),
-    ("reserved", "<u4", (64 - 23 - 2 * SEC_COUNT,)),
+    ("mc_tile_count", "<u4", (5,)), ("reserved", "<u4", (64 - 28 - 2 * SEC_COUNT,)),
 ])
 tu_dt = np.dtype([("x", "<u2"), ("y", "<u2"), ("plane", "u1"), ("log2", "u1"), ("kind", "u1"), ("flags", "u1"),
                   ("col_limit", "u1"), ("pad", "u1"), ("nnz", "<u2"), ("coeff_off", "<u4")])
@@ -37,7 +41,9 @@ mc_dt = np.dtype([("x", "<u2"), ("y", "<u2"), ("w", "u1"), ("h", "u1"), ("plane"
                   ("denom", "u1"), ("pad", "u1", (3,))])
 sao_dt = np.dtype([("type", "u1"), ("param", "u1"), ("borders", "u1"), ("edges", "u1"), ("variant", "u1"), ("tqb", "u1"),
                    ("offset_val", "<i2", (5,))])
-assert header_dt.itemsize == 256 and tu_dt.itemsize == 16 and intra_dt.itemsize == 16 and mc_dt.itemsize == 32 and sao_dt.itemsize == 16
+ccp_dt = np.dtype([("x", "<u2"), ("y", "<u2"), ("plane", "u1"), ("log2", "u1"), ("scale", "i1"), ("flags", "u1"),
+                   ("off_y", "<u4"), ("off_c", "<u4"), ("off_out", "<u4"), ("pad", "<u4", (3,))])
+cip_header_dt = np.dtype([("log2_min_pu_size", "<u4"), ("min_pu_width", "<u4"), ("min_pu_height", "<u4"), ("reserved", "<u4")])
 
 DBK_PRESENT = 0x8000
 
@@ -72,7 +78,7 @@ class DbkLayout:
 
 
 def split_mc_tiles(recs):
-    """Same tiling as b200_rec_mc(): every block becomes tiles of <= 16x16 (blocks taller than 8) or <= 32x8 samples (vectorised per block shape)."""
+    """The cut of B200_MC_TILE_WMAX / _HMAX (k_mc_expand): every block becomes tiles of <= 16x16 (blocks taller than 8) or <= 32x8 samples."""
     if len(recs) == 0:
         return np.zeros(0, mc_dt)
     out = []
@@ -96,8 +102,8 @@ def split_mc_tiles(recs):
 
 
 def order_mc(recs):
-    """B200_SEC_MC order (B200BlobHeader.mc_big_count): big tiles in the given order, then the <= 8x8 tiles bucketed by
-    (chroma, bi) -- same stable bucketing as b200_rec_finish().  Returns (ordered records, mc_big_count)."""
+    """B200_SEC_MC order of a tile list (B200BlobHeader.mc_big_count): big tiles in the given order, then the <= 8x8 tiles
+    stably bucketed by B200_MC_SMALL_KEY (chroma, bi), so that the tiles sharing a warp take the same branches.  Returns (ordered records, mc_big_count)."""
     recs = np.ascontiguousarray(recs, mc_dt)
     small = (recs["w"] <= 8) & (recs["h"] <= 8)
     key = np.where(small, 1 + np.where(recs["flags"] & MCF_CHROMA, 2, 0) + np.where(recs["flags"] & MCF_BI, 1, 0), 0)
@@ -123,7 +129,6 @@ def tu_dense(t, pool):
 def level_order(intra, width, height, cfi):
     """Permutation that sorts decode-order intra records by dependency level (stable) -- computed by the same host
     routine the C recorder uses (b200_intra_level_order in libb200hevc.so; pure host code, no GPU needed)."""
-    from . import _lib
     lib = _lib.load()
     intra = np.ascontiguousarray(intra, intra_dt)
     perm = np.zeros(len(intra), np.uint32)
@@ -131,6 +136,14 @@ def level_order(intra, width, height, cfi):
     if rc < 0:
         raise ValueError(f"b200_intra_level_order failed: {rc}")
     return perm, rc
+
+
+def _bitmap_section(log2_min_pu_size, bitmap):
+    """uint32 words of a CIP / TQB section: B200CipHeader, then one bit per min-PU of `bitmap` [min_pu_height, min_pu_width], row-major"""
+    bitmap = np.ascontiguousarray(bitmap, bool)
+    head = np.array([(log2_min_pu_size, bitmap.shape[1], bitmap.shape[0], 0)], cip_header_dt)
+    bits = np.packbits(bitmap.reshape(-1), bitorder="little")
+    return np.concatenate([head.view(np.uint8), bits, np.zeros(-len(bits) % 4, np.uint8)]).view("<u4")
 
 
 def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=None, tu=None, intra=None, mc=None,
@@ -159,30 +172,14 @@ def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=N
     hdr["mc_big_count"] = mc_big
     hdr["ref_slot"][0][:len(ref_slots)] = list(ref_slots)
     hdr["flags"] = (FRAME_HAS_DEBLOCK if len(parts[SEC_DBK]) else 0) | (FRAME_HAS_SAO if len(parts[SEC_SAO]) else 0)
-    off = 256
-    for s, p in enumerate(parts):
-        hdr["sec"][0][s] = (off, len(p))
-        off = (off + p.nbytes + 255) // 256 * 256
-    cip_words = None
+    extra = []                                   # optional sections behind the lists: (header field, uint32 words)
     if cip is not None:
-        log2_pu, bitmap = cip
-        bitmap = np.ascontiguousarray(bitmap, bool)
-        bits = np.packbits(bitmap.reshape(-1), bitorder="little")
-        bits = np.concatenate([bits, np.zeros(-len(bits) % 4, np.uint8)]).view("<u4")
-        cip_words = np.concatenate([np.array([log2_pu, bitmap.shape[1], bitmap.shape[0], 0], "<u4"), bits])
-        hdr["cip"][0] = (off, len(cip_words))
+        extra.append(("cip", _bitmap_section(*cip)))
         hdr["flags"] |= FRAME_CIP
-        off = (off + cip_words.nbytes + 255) // 256 * 256
-    tqb_words = None
     if tqb is not None and len(parts[SEC_SAO]):
-        log2_pu, bitmap = tqb
-        bitmap = np.ascontiguousarray(bitmap, bool)
-        bits = np.packbits(bitmap.reshape(-1), bitorder="little")
-        bits = np.concatenate([bits, np.zeros(-len(bits) % 4, np.uint8)]).view("<u4")
-        tqb_words = np.concatenate([np.array([log2_pu, bitmap.shape[1], bitmap.shape[0], 0], "<u4"), bits])
-        hdr["tqb"][0] = (off, len(tqb_words))
+        log2_pu, bitmap = tqb[0], np.asarray(tqb[1], bool)
+        extra.append(("tqb", _bitmap_section(log2_pu, bitmap)))
         hdr["flags"] |= FRAME_TQB
-        off = (off + tqb_words.nbytes + 255) // 256 * 256
         # mark the CTBs
         per = (1 << log2_ctb) >> log2_pu
         cw, ch = (width + (1 << log2_ctb) - 1) >> log2_ctb, (height + (1 << log2_ctb) - 1) >> log2_ctb
@@ -192,6 +189,15 @@ def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=N
                 if bitmap[cy * per:(cy + 1) * per, cx * per:(cx + 1) * per].any():
                     for pl in range(3):
                         g["tqb"][(pl * ch + cy) * cw + cx] = 1
+    off, placed = 256, []
+    for s, p in enumerate(parts):
+        hdr["sec"][0][s] = (off, len(p))
+        placed.append((off, p))
+        off = (off + p.nbytes + 255) // 256 * 256
+    for field, words in extra:
+        hdr[field][0] = (off, len(words))
+        placed.append((off, words))
+        off = (off + words.nbytes + 255) // 256 * 256
     hdr["total_bytes"] = off
     if out is None:
         out = np.zeros(off, np.uint8)
@@ -199,22 +205,20 @@ def build_blob(width, height, cfi, bit_depth, log2_ctb, cur_slot, poc=0, coeff=N
         assert out.dtype == np.uint8 and out.size >= off
         out = out[:off]
     out[:256] = hdr.view(np.uint8)
-    for s, p in enumerate(parts):
-        o = int(hdr["sec"][0][s]["off"])
+    for o, p in placed:
         out[o:o + p.nbytes] = p.view(np.uint8).reshape(-1)
-    if cip_words is not None:
-        o = int(hdr["cip"][0]["off"])
-        out[o:o + cip_words.nbytes] = cip_words.view(np.uint8)
-    if tqb_words is not None:
-        o = int(hdr["tqb"][0]["off"])
-        out[o:o + tqb_words.nbytes] = tqb_words.view(np.uint8)
     return out
+
+
+def header(blob):
+    """the B200BlobHeader of a uint8 blob, as a view: writing a field patches the blob"""
+    return blob[:256].view(header_dt)[0]
 
 
 def parse_blob(blob):
     """Inverse of build_blob (views into the blob)."""
     blob = np.frombuffer(blob, np.uint8) if not isinstance(blob, np.ndarray) else blob
-    hdr = blob[:256].view(header_dt)[0]
+    hdr = header(blob)
     assert hdr["magic"] == MAGIC and hdr["version"] == VERSION
     dts = [np.int16, tu_dt, tu_dt, tu_dt, tu_dt, intra_dt, mc_dt, np.uint16, sao_dt]
     secs = []
@@ -222,3 +226,85 @@ def parse_blob(blob):
         o, n = int(hdr["sec"][s]["off"]), int(hdr["sec"][s]["count"])
         secs.append(blob[o:o + n * np.dtype(dts[s]).itemsize].view(dts[s]))
     return hdr, secs
+
+
+class Recorder:
+    """The C recorder (b200_rec_*, include/b200hevc.h) recording one picture of a geometry (width, height, chroma_format_idc,
+    bit_depth): one method per table call.  A call the library refuses raises B200Error with its B200_E* code.  finish()
+    returns a copy of the blob; the C recorder is released then, or when the object goes away."""
+
+    def __init__(self, geom, cur_slot=0, poc=0):
+        self.lib, self.r = _lib.load(), C.c_void_p()
+        w, h, cfi, bd = geom
+        cfg = _lib.B200Config(width=w, height=h, chroma_format_idc=cfi, bit_depth=bd, log2_ctb_size=6)
+        rc = self.lib.b200_rec_create(C.byref(cfg), C.byref(self.r))
+        if rc:
+            raise B200Error(f"b200_rec_create failed ({rc})", rc)
+        self.begin(cur_slot, poc)
+
+    def _call(self, name, *args):
+        """the arrays behind the addresses in `args` must be held by the caller until the call returns"""
+        rc = getattr(self.lib, "b200_rec_" + name)(self.r, *args)
+        if rc:
+            raise B200Error(f"b200_rec_{name} failed ({rc})", rc)
+
+    def begin(self, cur_slot, poc=0):
+        self._call("begin", cur_slot, poc)
+
+    def set_refs(self, slots):
+        self._call("set_refs", bytes(slots), len(slots))
+
+    def tu(self, plane, x, y, log2, kind, flags, col_limit, coeffs, linked):
+        c = np.ascontiguousarray(coeffs, np.int16)
+        self._call("tu", plane, x, y, log2, kind, flags, col_limit, c.ctypes.data, linked)
+
+    def tu_parked(self, plane, x, y, log2, kind, flags, col_limit, coeffs):
+        c, off = np.ascontiguousarray(coeffs, np.int16), C.c_uint32()
+        self._call("tu_parked", plane, x, y, log2, kind, flags, col_limit, c.ctypes.data, C.byref(off))
+        return off.value
+
+    def pcm(self, plane, x, y, log2, samples):
+        s = np.ascontiguousarray(samples, np.int16)
+        self._call("pcm", plane, x, y, log2, s.ctypes.data)
+
+    def intra(self, plane, x, y, log2, mode, flags, top_right_size, bottom_left_size):
+        self._call("intra", plane, x, y, log2, mode, flags, top_right_size, bottom_left_size)
+
+    def mc(self, block):
+        b = np.ascontiguousarray(block, mc_dt)
+        self._call("mc", b.ctypes.data)
+
+    def deblock(self, plane, vertical, x, y, beta, tc, no_p, no_q):
+        self._call("deblock", plane, vertical, x, y, beta, (C.c_int * 2)(*tc), (C.c_uint8 * 2)(*no_p), (C.c_uint8 * 2)(*no_q))
+
+    def sao(self, plane, x, y, params):
+        p = np.ascontiguousarray(params, sao_dt)
+        self._call("sao", plane, x, y, p.ctypes.data)
+
+    def set_cip(self, log2_min_pu_size, is_intra):
+        """is_intra: array [min_pu_height, min_pu_width], non-zero = intra PU"""
+        m = np.ascontiguousarray(is_intra, np.uint8)
+        self._call("set_cip", log2_min_pu_size, m.shape[1], m.shape[0], m.ctypes.data)
+
+    def ccp(self, plane, x, y, log2, scale, off_y, has_c, off_c):
+        self._call("ccp", plane, x, y, log2, scale, off_y, has_c, off_c)
+
+    def merge(self, worker):
+        """fold the lists of `worker`, a Recorder of the same picture, into this one"""
+        self._call("merge", worker.r)
+
+    def finish(self):
+        try:
+            blob, nbytes = C.c_void_p(), C.c_uint64()
+            self._call("finish", C.byref(blob), C.byref(nbytes))
+            return np.ctypeslib.as_array(C.cast(blob, C.POINTER(C.c_uint8)), (nbytes.value,)).copy()
+        finally:
+            self.close()
+
+    def close(self):
+        if getattr(self, "r", None):
+            self.lib.b200_rec_destroy(self.r)
+            self.r = None
+
+    def __del__(self):
+        self.close()

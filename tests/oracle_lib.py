@@ -1,14 +1,18 @@
-"""TEST INFRASTRUCTURE: ctypes access to the CPU oracle (oracle/hevc_oracle.c) and helpers that
-compare the CUDA path with it.  Never imported by the product package."""
+"""TEST INFRASTRUCTURE: ctypes access to the CPU oracle (oracle/hevc_oracle.c), the numpy restatement of the colour
+conversion, and helpers that compare the CUDA path with them.  Never imported by the product package."""
 import ctypes as C
 import glob
 import hashlib
 import io
 import lzma
+import math
 import os
 import subprocess
 
 import numpy as np
+
+from openhevc_b200 import FrameEngine, _lib as b200_lib
+from openhevc_b200 import worklist as W
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_DIR = os.path.join(ROOT, "oracle")
@@ -44,8 +48,7 @@ def execute(blob, dpb):
     rc = lib().orc_execute_blob(blob.ctypes.data, ptrs, len(dpb))
     if rc:
         raise RuntimeError(f"orc_execute_blob failed: {rc}")
-    cur = int(blob[23])
-    return planes16[cur]
+    return planes16[int(W.header(blob)["cur_slot"])]
 
 
 REPLAY_SO = os.path.join(ORACLE_DIR, "_ref", "libreplay_ref.so")
@@ -71,8 +74,8 @@ def ref_lib():
     return _ref
 
 
-def _native(dpb, bit_depth):
-    dt = np.uint16 if bit_depth > 8 else np.uint8
+def _native(dpb, blob):
+    dt = np.uint16 if W.header(blob)["bit_depth"] > 8 else np.uint8
     planes = [[np.ascontiguousarray(p, dt).copy() for p in slot] for slot in dpb]
     flat = [p for slot in planes for p in slot]
     ptrs = (C.c_void_p * len(flat))(*[p.ctypes.data for p in flat])
@@ -83,11 +86,11 @@ def _native(dpb, bit_depth):
 def ref_execute(blob, dpb):
     """same contract as execute(), computed by the reference's own C functions"""
     blob = np.ascontiguousarray(blob, np.uint8)
-    planes, ptrs, strides = _native(dpb, int(blob[21]))
+    planes, ptrs, strides = _native(dpb, blob)
     rc = ref_lib().ref_execute_blob(blob.ctypes.data, ptrs, strides, len(dpb))
     if rc:
         raise RuntimeError(f"ref_execute_blob failed: {rc}")
-    return planes[int(blob[23])]
+    return planes[int(W.header(blob)["cur_slot"])]
 
 
 SHIM_SO = os.path.join(ORACLE_DIR, "_ref", "libb200hevc_shim.so")
@@ -97,7 +100,7 @@ def ref_execute_b200(blob, dpb):
     """The reference-side call sequence (oracle/replay_ref.c) issued through the B200 drop-in tables
     (libb200hevc_shim.so -> recorder -> GPU -> readback).  Needs a GPU."""
     blob = np.ascontiguousarray(blob, np.uint8)
-    planes, ptrs, strides = _native(dpb, int(blob[21]))
+    planes, ptrs, strides = _native(dpb, blob)
     L = ref_lib()
     L.ref_execute_blob_b200.restype = C.c_int
     L.ref_execute_blob_b200.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int, C.c_char_p, C.c_char_p, C.c_int]
@@ -105,13 +108,13 @@ def ref_execute_b200(blob, dpb):
     rc = L.ref_execute_blob_b200(blob.ctypes.data, ptrs, strides, len(dpb), SHIM_SO.encode(), err, 512)
     if rc:
         raise RuntimeError(f"ref_execute_blob_b200 failed: {rc}: {err.value.decode()}")
-    return planes[int(blob[23])]
+    return planes[int(W.header(blob)["cur_slot"])]
 
 
 def ref_bench(blobs, dpb, n_threads, iters):
     """seconds of wall time for n_threads x iters pictures on the reference C path"""
     blobs = [np.ascontiguousarray(b, np.uint8) for b in blobs]
-    planes, ptrs, strides = _native(dpb, int(blobs[0][21]))
+    planes, ptrs, strides = _native(dpb, blobs[0])
     bp = (C.c_void_p * len(blobs))(*[b.ctypes.data for b in blobs])
     t = ref_lib().ref_bench(bp, len(blobs), ptrs, strides, len(dpb), n_threads, iters)
     if t < 0:
@@ -126,10 +129,36 @@ def ref_bench_stages():
     return dict(zip(("mc", "residual", "intra", "deblock", "sao"), [float(v) for v in out]))
 
 
+def assert_same(got, want, what):
+    for p in range(3):
+        assert np.shape(got[p]) == np.shape(want[p]), f"{what} plane {p}: shape {np.shape(got[p])}, want {np.shape(want[p])}"
+        bad = np.argwhere(np.asarray(got[p]) != np.asarray(want[p]))
+        assert len(bad) == 0, f"{what} plane {p}: {len(bad)} samples differ, first at (y,x)={tuple(bad[0])} got {got[p][tuple(bad[0])]} want {want[p][tuple(bad[0])]}"
+
+
+def padded_engine(geom, n_slots, **kw):
+    """a FrameEngine on a caller-owned DPB (ext_frame_mem) whose every byte starts as 0x5a: garbage in the row padding of
+    each slot, which no kernel may read.  A torch CUDA tensor on the device; the emulated library's device memory is host
+    memory, so there a numpy buffer."""
+    cfg = b200_lib.B200Config(0, *geom, 6, n_slots, 2, 0, None, 0)
+    nbytes = int(b200_lib.load().b200_dpb_bytes(C.byref(cfg)))
+    if "_emul" in os.path.basename(b200_lib.LIB_PATH):
+        raw = np.full(nbytes + 256, 0x5a, np.uint8)
+        mem = raw[-raw.ctypes.data % 256:][:nbytes]                   # ext_frame_mem must be 256-byte aligned
+        ptr = mem.ctypes.data
+    else:
+        import torch
+        mem = torch.full((nbytes,), 0x5a, dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        ptr = mem.data_ptr()
+    eng = FrameEngine(*geom, n_slots=n_slots, ext_frame_mem=ptr, ext_frame_bytes=nbytes, **kw)
+    eng.dpb_mem = mem                                                  # the engine does not own it: keep it alive as long
+    return eng
+
+
 def check_decode_order(blob):
     """host-side validation of a blob's intra list: every neighbour unit an intra TU reads must be final
     (not covered by a *later* intra TU).  A violation would make the device wavefront wait forever."""
-    from openhevc_b200 import worklist as W
     hdr, secs = W.parse_blob(blob)
     intra = secs[W.SEC_INTRA]
     w, h, cfi = int(hdr["width"]), int(hdr["height"]), int(hdr["chroma_format_idc"])
@@ -157,6 +186,12 @@ def check_decode_order(blob):
     return True
 
 
+# A stream with a conformance window (coded 432x256, output 416x240, non-zero left and top offsets).  It lives apart from
+# golden/streams/: the tests over that directory compare whole coded pictures.  For a window with a top (or left) offset the
+# decoder's output frame points INSIDE its buffer (ff_hevc_output_frame moves the data pointers), so the shim has to find the
+# read-back of such a frame by range, not by its first byte: with frame threads the frame is output before it has landed.
+CROPPED = os.path.join(ROOT, "tests", "golden", "streams_cropped", "crop_432x256_10b_lowdelay.hevc")
+
 WORKLIST_DIR = os.path.join(ROOT, "tests", "golden", "worklists")
 
 
@@ -183,12 +218,10 @@ def recorded_worklists(stream, threads="1"):
 
 def replay_worklists(rec, gpu):
     """recorded work lists in decode order on one DPB, by the CUDA path or the CPU oracle: {output index: md5_line}"""
-    from openhevc_b200 import worklist as W
     hdr, _ = W.parse_blob(rec["blobs"][0])
     w, h, cfi, bd = int(hdr["width"]), int(hdr["height"]), int(hdr["chroma_format_idc"]), int(hdr["bit_depth"])
     n_slots, lines = 32, {}
     if gpu:
-        from openhevc_b200 import FrameEngine
         eng = FrameEngine(w, h, cfi, bd, log2_ctb_size=int(hdr["log2_ctb_size"]), n_slots=n_slots)
     else:
         dpb = [[np.zeros(W.plane_dims(w, h, cfi, p)[::-1], np.uint16) for p in range(3)] for _ in range(n_slots)]
@@ -216,3 +249,44 @@ def recorded_streams():
     import zipfile
     names = [n for p in glob.glob(os.path.join(WORKLIST_DIR, "pack_*.zip")) for n in zipfile.ZipFile(p).namelist()]
     return sorted(os.path.join(ROOT, "tests", "golden", "streams", n[:-7] + ".hevc") for n in names if n.count(".") == 2)
+
+
+# the fixed-point colour conversion of openhevc_b200/csrc/k_yuv_rgb.cuh restated in numpy: the kernel must equal it bit for bit
+KR_KB = {1: (0.2126, 0.0722), 5: (0.299, 0.114), 6: (0.299, 0.114), 9: (0.2627, 0.0593)}
+
+
+def yuv_rgb_coef(matrix, full_range, bd, out_float):
+    """(cy, crv, cgu, cgv, cbu, yoff, coff, W, scale): the Q13 coefficients of k_yuv_rgb.cuh, same operations in the same order"""
+    kr, kb = KR_KB[matrix]
+    kg = 1.0 - kr - kb
+    W = (1 << bd) - 1 if out_float else 255
+    sy = W / float((1 << bd) - 1) if full_range else W / float(219 << (bd - 8))
+    sc = W / float((1 << bd) - 1) if full_range else W / float(224 << (bd - 8))
+
+    def q(x):
+        return int(math.floor(x * 8192.0 + 0.5))
+    return (q(sy), q(2.0 * (1.0 - kr) * sc), q(2.0 * kb * (1.0 - kb) / kg * sc), q(2.0 * kr * (1.0 - kr) / kg * sc),
+            q(2.0 * (1.0 - kb) * sc), 0 if full_range else 16 << (bd - 8), 1 << (bd - 1), W,
+            np.float32(1.0 / W) if out_float else np.float32(1.0))
+
+
+def yuv_rgb_reference(planes, cfi, bd, matrix, full_range, out_float, crop):
+    cy, crv, cgu, cgv, cbu, yoff, coff, W, scale = yuv_rgb_coef(matrix, full_range, bd, out_float)
+    x0, y0, w, h = crop
+    sx, sy = int(cfi != 3), int(cfi == 1)
+    ys, xs = np.mgrid[y0:y0 + h, x0:x0 + w]
+    Y = planes[0][ys, xs].astype(np.int64)
+    U = planes[1][ys >> sy, xs >> sx].astype(np.int64) - coff
+    V = planes[2][ys >> sy, xs >> sx].astype(np.int64) - coff
+    lum = cy * (Y - yoff) + 4096
+    rgb = np.stack([np.clip((lum + crv * V) >> 13, 0, W), np.clip((lum - cgu * U - cgv * V) >> 13, 0, W),
+                    np.clip((lum + cbu * U) >> 13, 0, W)])
+    assert np.abs(lum).max() < 2 ** 31 and np.abs(lum + crv * V).max() < 2 ** 31      # the kernel accumulates in int32
+    return rgb.astype(np.float32) * scale if out_float else rgb.astype(np.uint8)
+
+
+def random_planes(w, h, cfi, bd, seed):
+    rng = np.random.default_rng(seed)
+    sx, sy = int(cfi != 3), int(cfi == 1)
+    dt = np.uint16 if bd > 8 else np.uint8
+    return [rng.integers(0, 1 << bd, size=s, dtype=np.int64).astype(dt) for s in ((h, w), (h >> sy, w >> sx), (h >> sy, w >> sx))]

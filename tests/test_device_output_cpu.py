@@ -1,10 +1,9 @@
 """CPU suite for device-resident output: b200_yuv_to_rgb (k_yuv_rgb) and b200_slot_export_async, run on the warp-lockstep
 emulated library (oracle/_ref/libb200hevc_emul.so: kernels.cu + engine.cu compiled unchanged for the CPU).
 
-yuv_rgb_reference() restates the fixed-point definition of openhevc_b200/csrc/k_yuv_rgb.cuh in numpy; the kernel must equal it
-bit for bit, for uint8 and for float32 output."""
+oracle_lib.yuv_rgb_reference() restates the fixed-point definition of openhevc_b200/csrc/k_yuv_rgb.cuh in numpy; the kernel must
+equal it bit for bit, for uint8 and for float32 output."""
 import ctypes as C
-import math
 import os
 import subprocess
 import sys
@@ -12,50 +11,13 @@ import sys
 import numpy as np
 import pytest
 
+from oracle_lib import CROPPED, random_planes, yuv_rgb_reference
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 REFDIR = os.path.join(ROOT, "oracle", "_ref")
 EMUL = os.path.join(REFDIR, "libb200hevc_emul.so")
 needs_emul = pytest.mark.skipif(not os.path.exists(EMUL), reason="oracle/_ref/libb200hevc_emul.so not built (make -C tests/emul)")
-
-KR_KB = {1: (0.2126, 0.0722), 5: (0.299, 0.114), 6: (0.299, 0.114), 9: (0.2627, 0.0593)}
-
-
-def yuv_rgb_coef(matrix, full_range, bd, out_float):
-    """(cy, crv, cgu, cgv, cbu, yoff, coff, W, scale): the Q13 coefficients of k_yuv_rgb.cuh, same operations in the same order"""
-    kr, kb = KR_KB[matrix]
-    kg = 1.0 - kr - kb
-    W = (1 << bd) - 1 if out_float else 255
-    sy = W / float((1 << bd) - 1) if full_range else W / float(219 << (bd - 8))
-    sc = W / float((1 << bd) - 1) if full_range else W / float(224 << (bd - 8))
-
-    def q(x):
-        return int(math.floor(x * 8192.0 + 0.5))
-    return (q(sy), q(2.0 * (1.0 - kr) * sc), q(2.0 * kb * (1.0 - kb) / kg * sc), q(2.0 * kr * (1.0 - kr) / kg * sc),
-            q(2.0 * (1.0 - kb) * sc), 0 if full_range else 16 << (bd - 8), 1 << (bd - 1), W,
-            np.float32(1.0 / W) if out_float else np.float32(1.0))
-
-
-def yuv_rgb_reference(planes, cfi, bd, matrix, full_range, out_float, crop):
-    cy, crv, cgu, cgv, cbu, yoff, coff, W, scale = yuv_rgb_coef(matrix, full_range, bd, out_float)
-    x0, y0, w, h = crop
-    sx, sy = int(cfi != 3), int(cfi == 1)
-    ys, xs = np.mgrid[y0:y0 + h, x0:x0 + w]
-    Y = planes[0][ys, xs].astype(np.int64)
-    U = planes[1][ys >> sy, xs >> sx].astype(np.int64) - coff
-    V = planes[2][ys >> sy, xs >> sx].astype(np.int64) - coff
-    lum = cy * (Y - yoff) + 4096
-    rgb = np.stack([np.clip((lum + crv * V) >> 13, 0, W), np.clip((lum - cgu * U - cgv * V) >> 13, 0, W),
-                    np.clip((lum + cbu * U) >> 13, 0, W)])
-    assert np.abs(lum).max() < 2 ** 31 and np.abs(lum + crv * V).max() < 2 ** 31      # the kernel accumulates in int32
-    return rgb.astype(np.float32) * scale if out_float else rgb.astype(np.uint8)
-
-
-def random_planes(w, h, cfi, bd, seed):
-    rng = np.random.default_rng(seed)
-    sx, sy = int(cfi != 3), int(cfi == 1)
-    dt = np.uint16 if bd > 8 else np.uint8
-    return [rng.integers(0, 1 << bd, size=s, dtype=np.int64).astype(dt) for s in ((h, w), (h >> sy, w >> sx), (h >> sy, w >> sx))]
 
 
 def run_yuv_rgb(lib, planes, cfi, bd, matrix, full_range, out_float, crop):
@@ -232,13 +194,6 @@ def test_export_rejects_crop_windows_off_the_chroma_grid():
         assert eng.lib.b200_slot_export_async(eng.h, 0, C.byref(e), None) == 0      # the rejected calls left the context usable
     finally:
         eng.close()
-
-
-# A stream with a conformance window (coded 432x256, output 416x240, non-zero left and top offsets).  It lives apart from
-# golden/streams/: the tests over that directory compare whole coded pictures.  For a window with a top (or left) offset the
-# decoder's output frame points INSIDE its buffer (ff_hevc_output_frame moves the data pointers), so the shim has to find the
-# read-back of such a frame by range, not by its first byte: with frame threads the frame is output before it has landed.
-CROPPED = os.path.join(HERE, "golden", "streams_cropped", "crop_432x256_10b_lowdelay.hevc")
 
 
 @needs_emul

@@ -1,12 +1,12 @@
 """Device-resident output on the GPU: FrameEngine.export (b200_slot_export_async) ordered as a slot reader, and yuv_to_rgb
-(k_yuv_rgb) against the numpy restatement of its fixed-point definition (test_device_output_cpu.yuv_rgb_reference)."""
+(k_yuv_rgb) against the numpy restatement of its fixed-point definition (oracle_lib.yuv_rgb_reference)."""
 import os
 
 import numpy as np
 import pytest
 
 import oracle_lib
-from test_device_output_cpu import random_planes, yuv_rgb_reference
+from oracle_lib import CROPPED, random_planes, yuv_rgb_reference
 
 pytestmark = pytest.mark.gpu
 STREAMS = oracle_lib.recorded_streams()
@@ -115,8 +115,7 @@ def test_yuv_to_rgb_small_pictures(cfi, bd):
 def test_cropped_stream_through_the_hooked_decoder(threads):
     """the host read-back path on a stream with a conformance window (output frames point inside their buffers)"""
     import subprocess
-    from test_device_output_cpu import CROPPED, REFDIR
-    decoder = os.path.join(REFDIR, "decode_b200")
+    decoder = os.path.join(oracle_lib.ORACLE_DIR, "_ref", "decode_b200")
     if not os.path.exists(decoder):
         pytest.skip("oracle/_ref/decode_b200 not built")
     out = subprocess.run([decoder, CROPPED, threads], capture_output=True, text=True, timeout=600)

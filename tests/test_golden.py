@@ -26,9 +26,7 @@ def test_fixtures_exist():
 @pytest.mark.parametrize("path", FIXTURES, ids=[os.path.basename(p) for p in FIXTURES])
 def test_oracle_reproduces_reference_golden(path):
     blob, geom, dpb, want = load(path)
-    got = oracle_lib.execute(blob, dpb)
-    for p in range(3):
-        assert (got[p] == want[p]).all()
+    oracle_lib.assert_same(oracle_lib.execute(blob, dpb), want, os.path.basename(path))
 
 
 @pytest.mark.gpu
@@ -40,8 +38,6 @@ def test_cuda_reproduces_reference_golden(path):
     try:
         for s in (1, 2):
             eng.upload_slot(s, dpb[s])
-        got = eng.decode(blob)
-        for p in range(3):
-            assert (got[p] == want[p]).all()
+        oracle_lib.assert_same(eng.decode(blob), want, os.path.basename(path))
     finally:
         eng.close()

@@ -11,10 +11,9 @@ import numpy as np
 import pytest
 
 import oracle_lib
+from oracle_lib import assert_same, padded_engine
 from openhevc_b200 import worklist as W
 from openhevc_b200.synth import smooth_frame
-from test_mc_limits_gpu import padded_engine
-from test_residual_intra_limits_gpu import Recorder, assert_same
 
 pytestmark = pytest.mark.gpu
 
@@ -22,7 +21,7 @@ pytestmark = pytest.mark.gpu
 def pcm_picture(geom, planes):
     """coeff / tu sections of a blob whose residual stage writes `planes` as PCM blocks (the largest that fit, up to 32x32)"""
     w, h, cfi, bd = geom
-    rec = Recorder(geom)
+    rec = W.Recorder(geom)
 
     def quad(p, x, y, log2):
         pw, ph = W.plane_dims(w, h, cfi, p)

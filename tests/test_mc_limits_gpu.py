@@ -8,14 +8,12 @@ beyond every picture border.  Each picture runs twice on the device: as a list o
 whole prediction blocks that the device cuts into tiles (k_mc_expand; recorded through the C recorder, b200_rec_mc).  Both
 must equal the CPU oracle, and where the reference's own tables are built (oracle/_ref/libreplay_ref.so) the oracle must equal
 them as well.  Destination rectangles within a picture never overlap, so the order in which tiles run cannot matter."""
-import ctypes as C
-import os
-
 import numpy as np
 import pytest
 
 import oracle_lib
-from openhevc_b200 import FrameEngine, B200Error, _lib
+from oracle_lib import assert_same, padded_engine
+from openhevc_b200 import FrameEngine, B200Error
 from openhevc_b200 import worklist as W
 from openhevc_b200.synth import FrameSynth, smooth_frame
 
@@ -193,22 +191,11 @@ def assert_list0_wraps(pictures, bd):
 def block_blob(geom, recs, cur_slot=0, poc=0):
     """the records as whole prediction blocks through the C recorder, the way the decoder's table calls arrive (b200_rec_mc):
     the blob carries B200BlobHeader.mc_tile_count and the device cuts the blocks into tiles itself (k_mc_expand)"""
-    lib = _lib.load()
-    width, height, cfi, bd = geom
-    cfg = _lib.B200Config(0, width, height, cfi, bd, 6, 3, 2, 0, None, 0)
-    r = C.c_void_p()
-    assert lib.b200_rec_create(C.byref(cfg), C.byref(r)) == 0
-    try:
-        assert lib.b200_rec_begin(r, cur_slot, poc) == 0
-        for k in range(len(recs)):
-            one = np.ascontiguousarray(recs[k:k + 1], W.mc_dt)
-            assert lib.b200_rec_mc(r, one.ctypes.data) == 0
-        assert lib.b200_rec_set_refs(r, bytes(REF_SLOTS), len(REF_SLOTS)) == 0
-        bp, nb = C.c_void_p(), C.c_uint64()
-        assert lib.b200_rec_finish(r, C.byref(bp), C.byref(nb)) == 0
-        return np.ctypeslib.as_array(C.cast(bp, C.POINTER(C.c_uint8)), (nb.value,)).copy()
-    finally:
-        lib.b200_rec_destroy(r)
+    rec = W.Recorder(geom, cur_slot, poc)
+    for block in recs:
+        rec.mc(block)
+    rec.set_refs(REF_SLOTS)
+    return rec.finish()
 
 
 def tile_blob(geom, recs):
@@ -226,12 +213,6 @@ def assert_disjoint(geom, recs):
         assert cover.max() <= 1, f"plane {p}: destinations overlap"
 
 
-def assert_same(got, want, what):
-    for p in range(3):
-        bad = np.argwhere(np.asarray(got[p]) != np.asarray(want[p]))
-        assert len(bad) == 0, f"{what} plane {p}: {len(bad)} samples differ, first at (y,x)={tuple(bad[0])} got {got[p][tuple(bad[0])]} want {want[p][tuple(bad[0])]}"
-
-
 def check_picture(eng, geom, recs, dpb, what, reference_tables=True, blobs=None):
     """tile form and block form on the device, against the oracle (and the oracle against the reference's tables)"""
     assert_disjoint(geom, recs)
@@ -245,27 +226,6 @@ def check_picture(eng, geom, recs, dpb, what, reference_tables=True, blobs=None)
     for blob, form in ((tiles, "tile form"), (blocks, "block form")):
         eng.upload_slot(0, dpb[0])
         assert_same(eng.decode(blob), want, f"{what} {form}")
-
-
-def padded_engine(geom, n_slots, **kw):
-    """a FrameEngine on a caller-owned DPB (ext_frame_mem) whose every byte starts as 0x5a: garbage in the row padding of
-    each slot, which no kernel may read.  A torch CUDA tensor on the device; the emulated library's device memory is host
-    memory, so there a numpy buffer."""
-    width, height, cfi, bd = geom
-    cfg = _lib.B200Config(0, width, height, cfi, bd, 6, n_slots, 2, 0, None, 0)
-    nbytes = int(_lib.load().b200_dpb_bytes(C.byref(cfg)))
-    if "_emul" in os.path.basename(_lib.LIB_PATH):
-        raw = np.full(nbytes + 256, 0x5a, np.uint8)
-        mem = raw[-raw.ctypes.data % 256:][:nbytes]                   # ext_frame_mem must be 256-byte aligned
-        ptr = mem.ctypes.data
-    else:
-        import torch
-        mem = torch.full((nbytes,), 0x5a, dtype=torch.uint8, device="cuda")
-        torch.cuda.synchronize()
-        ptr = mem.data_ptr()
-    eng = FrameEngine(*geom, n_slots=n_slots, ext_frame_mem=ptr, ext_frame_bytes=nbytes, **kw)
-    eng.dpb_mem = mem                                                  # the engine does not own it: keep it alive as long
-    return eng
 
 
 def run_sweep(geom, contents, rects_per_picture, seed, wrap_guard=True):
@@ -378,7 +338,7 @@ def test_small_tile_region_need_not_be_bucket_ordered():
 
 
 @pytest.mark.late
-def test_malformed_block_lists_are_rejected_on_the_device():
+def test_block_lists_whose_tile_counts_or_places_disagree_are_rejected():
     """A block-form list says where each block's tiles go in the lane's tile list (B200McRec.pad, per bucket; the header's
     mc_tile_count sizes the buckets).  A header that claims more tiles than its blocks cut into, or two blocks that claim the
     same place, leave places unwritten -- and on a lane that ran a picture of the same geometry before, those places still hold
@@ -396,19 +356,19 @@ def test_malformed_block_lists_are_rejected_on_the_device():
             eng.upload_slot(slot, dpb[slot])
         good = block_blob(geom, recs)
         hdr, secs = W.parse_blob(good)
-        assert list(hdr["reserved"][:5]) == [4, 1, 1, 0, 0] and list(secs[W.SEC_MC]["pad"][:3, 0]) == [0, 2, 3]
+        assert list(hdr["mc_tile_count"]) == [4, 1, 1, 0, 0] and list(secs[W.SEC_MC]["pad"][:3, 0]) == [0, 2, 3]
         eng.upload_slot(0, dpb[0])
         first = eng.decode(good)
         assert_same(first, oracle_lib.execute(good, dpb), "good block list")
         # 1. C left out, the header still counts its tile: place 3 keeps C's tile from the picture before
         bad = block_blob(geom, recs[[0, 1, 3, 4]])
-        bad[:256].view(W.header_dt)["reserved"][0][0] += 1
+        W.header(bad)["mc_tile_count"][0] += 1
         # 2. C claims B's place: place 3 is not written
         bad2 = good.copy()
         W.parse_blob(bad2)[1][W.SEC_MC]["pad"][2] = W.parse_blob(bad2)[1][W.SEC_MC]["pad"][1]
         # 3. the same, with the header counting only the places the blocks cover: every place is written, one of them twice
         bad3 = bad2.copy()
-        bad3[:256].view(W.header_dt)["reserved"][0][0] -= 1
+        W.header(bad3)["mc_tile_count"][0] -= 1
         for k, blob in enumerate((bad, bad2, bad3)):
             eng.upload_slot(0, dpb[0])
             with pytest.raises(B200Error, match="rejected on the device"):

@@ -32,6 +32,27 @@ def test_blob_roundtrip_and_layout():
     assert len(secs[W.SEC_DBK]) == L.total
 
 
+def test_numpy_mirror_matches_the_c_header(tmp_path):
+    """every field of every dtype of worklist.py at the offset and with the size the C compiler gives the struct field of the
+    same name in include/b200hevc_worklist.h, every struct of the same size, and every constant of the same value"""
+    lines, want = [], []
+    for struct, dt in {"B200Section": W.section_dt, "B200BlobHeader": W.header_dt, "B200TuRec": W.tu_dt, "B200IntraRec": W.intra_dt, "B200McRec": W.mc_dt,
+                       "B200SaoRec": W.sao_dt, "B200CcpRec": W.ccp_dt, "B200CipHeader": W.cip_header_dt}.items():
+        lines.append(f'printf("{struct} %zu\\n", sizeof({struct}));')
+        want.append(f"{struct} {dt.itemsize}")
+        for name, (fdt, off) in dt.fields.items():
+            lines.append(f'printf("{struct}.{name} %zu %zu\\n", offsetof({struct}, {name}), sizeof((({struct} *)0)->{name}));')
+            want.append(f"{struct}.{name} {off} {fdt.itemsize}")
+    for name, value in vars(W).items():
+        if name.isupper() and isinstance(value, int):
+            lines.append(f'printf("{name} %lld\\n", (long long)B200_{"BLOB_" if name in ("MAGIC", "VERSION") else ""}{name});')
+            want.append(f"{name} {value}")
+    src = tmp_path / "layout.c"
+    src.write_text("#include <stddef.h>\n#include <stdio.h>\n#include \"b200hevc_worklist.h\"\nint main(void)\n{\n" + "\n".join(lines) + "\nreturn 0;\n}\n")
+    subprocess.run(["cc", "-I", os.path.join(oracle_lib.ROOT, "include"), "-o", str(tmp_path / "layout"), str(src)], check=True)
+    assert subprocess.run([str(tmp_path / "layout")], capture_output=True, text=True, check=True).stdout.splitlines() == want
+
+
 @pytest.mark.parametrize("cfi,bd,refs", [(1, 8, []), (1, 10, [1, 2]), (2, 10, [1]), (3, 8, [1, 2])])
 def test_synth_is_in_decode_order_and_oracle_runs(cfi, bd, refs):
     w, h = 192, 128
@@ -60,10 +81,7 @@ def test_oracle_equals_reference_at_picture_level(built, cfi, bd, refs, kw):
     blob, st = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=90 + cfi + bd, refs=refs, cur_slot=0, exotic=0.05, max_mv=100, **kw).generate()
     dpb = [smooth_frame(w, h, cfi, bd, 200 + k) for k in range(3)]
     a = oracle_lib.execute(blob, dpb)
-    b = oracle_lib.ref_execute(blob, dpb)
-    for p in range(3):
-        bad = np.argwhere(a[p] != b[p])
-        assert len(bad) == 0, f"plane {p}: {len(bad)} differ, first {tuple(bad[0])}"
+    oracle_lib.assert_same(a, oracle_lib.ref_execute(blob, dpb), "oracle against the reference tables")
 
 
 def test_oracle_properties_linearity_of_residual():
@@ -124,20 +142,17 @@ def test_no_gpu_means_loud_failure_not_fallback(built):
         FrameEngine(64, 64)
 
 
-def replay_through_recorders(lib, blob, geom, n_workers):
+TU_ARGS = ("plane", "x", "y", "log2", "kind", "flags", "col_limit")
+
+
+def replay_through_recorders(blob, geom, n_workers):
     """Replays a blob's records through the C recorder the way the decoder's table calls would arrive.  With
     n_workers > 1 the calls of CTB row k go to recorder k % n_workers (WPP / slice threads: every worker has its own
     B200Rec and its own, lazily built reference table) and the workers are folded into recorder 0 with b200_rec_merge."""
-    from openhevc_b200 import _lib
     w, h, cfi, bd = geom
     hdr, secs = W.parse_blob(blob)
-    cfg = _lib.B200Config(0, w, h, cfi, bd, 6, 6, 2, 0, None, 0)
-    recs, tables = [], []
-    for k in range(n_workers):
-        r = C.c_void_p()
-        assert lib.b200_rec_create(C.byref(cfg), C.byref(r)) == 0
-        assert lib.b200_rec_begin(r, int(hdr["cur_slot"]), 0) == 0
-        recs.append(r); tables.append([])
+    recs = [W.Recorder(geom, int(hdr["cur_slot"])) for _ in range(n_workers)]
+    tables = [[] for _ in range(n_workers)]
 
     def who(plane, y):
         vs = 1 if (plane and cfi == 1) else 0
@@ -152,18 +167,15 @@ def replay_through_recorders(lib, blob, geom, n_workers):
                 parked[W.tu_dense(t, pool)[1]] = t
     for ir in secs[W.SEC_INTRA]:
         r = recs[who(ir["plane"], ir["y"])]
-        assert lib.b200_rec_intra(r, int(ir["plane"]), int(ir["x"]), int(ir["y"]), int(ir["log2"]), int(ir["mode"]), int(ir["flags"]),
-                                  int(ir["top_right_size"]), int(ir["bottom_left_size"])) == 0
+        r.intra(*(ir[f] for f in ("plane", "x", "y", "log2", "mode", "flags", "top_right_size", "bottom_left_size")))
         if ir["resid_off"] != W.NO_RESID:
             t = parked[int(ir["resid_off"])]
-            c = np.ascontiguousarray(W.tu_dense(t, pool)[0])
-            assert lib.b200_rec_tu(r, int(t["plane"]), int(t["x"]), int(t["y"]), int(t["log2"]), int(t["kind"]), int(t["flags"]), int(t["col_limit"]), c.ctypes.data, 1) == 0
+            r.tu(*(t[f] for f in TU_ARGS), W.tu_dense(t, pool)[0], 1)
     for k in range(4):
         for t in secs[W.SEC_TU4 + k]:
             if t["flags"] & W.TUF_PARK:
                 continue
-            c = np.ascontiguousarray(W.tu_dense(t, pool)[0])
-            assert lib.b200_rec_tu(recs[who(t["plane"], t["y"])], int(t["plane"]), int(t["x"]), int(t["y"]), int(t["log2"]), int(t["kind"]), int(t["flags"]), int(t["col_limit"]), c.ctypes.data, -1) == 0
+            recs[who(t["plane"], t["y"])].tu(*(t[f] for f in TU_ARGS), W.tu_dense(t, pool)[0], -1)
     ref_slots = [int(v) for v in hdr["ref_slot"][:int(hdr["n_ref"])]]
     for m in secs[W.SEC_MC]:
         k = who(m["plane"], m["y"])
@@ -173,7 +185,7 @@ def replay_through_recorders(lib, blob, geom, n_workers):
             if slot not in tables[k]:
                 tables[k].append(slot)
             mm[f] = tables[k].index(slot)
-        assert lib.b200_rec_mc(recs[k], mm.ctypes.data) == 0
+        recs[k].mc(mm)
     L = W.DbkLayout(w, h, cfi)
     grid = secs[W.SEC_DBK]
     for p in range(3):
@@ -188,40 +200,29 @@ def replay_through_recorders(lib, blob, geom, n_workers):
                     continue
                 done.add((x0, y0))
                 ent = [int(v[(y0 // 4 + j), gx]) if d == 0 else int(v[gy, x0 // 4 + j]) for j in range(2)]
-                tc = (C.c_int * 2)(*[e & 63 for e in ent])
-                nop = (C.c_uint8 * 2)(*[(e >> 13) & 1 for e in ent]); noq = (C.c_uint8 * 2)(*[(e >> 14) & 1 for e in ent])
                 beta = max((e >> 6) & 127 for e in ent)
-                assert lib.b200_rec_deblock(recs[who(p, y0)], p, 1 - d, x0, y0, beta, tc, nop, noq) == 0
+                recs[who(p, y0)].deblock(p, 1 - d, x0, y0, beta, [e & 63 for e in ent], [(e >> 13) & 1 for e in ent], [(e >> 14) & 1 for e in ent])
     sg = secs[W.SEC_SAO]
     nctb = len(sg) // 3
     cw = (w + 63) // 64
     for p in range(3):
         hs, vs = ((1 if cfi != 3 else 0), (1 if cfi == 1 else 0)) if p else (0, 0)
         for i in range(nctb):
-            e = np.array([sg[p * nctb + i]])
-            assert lib.b200_rec_sao(recs[(i // cw) % n_workers], p, ((i % cw) * 64) >> hs, ((i // cw) * 64) >> vs, e.ctypes.data) == 0
+            recs[(i // cw) % n_workers].sao(p, ((i % cw) * 64) >> hs, ((i // cw) * 64) >> vs, sg[p * nctb + i])
     for k in range(n_workers):
-        tab = tables[k]
-        assert lib.b200_rec_set_refs(recs[k], bytes(tab), len(tab)) == 0
+        recs[k].set_refs(tables[k])
     for k in range(1, n_workers):
-        assert lib.b200_rec_merge(recs[0], recs[k]) == 0
-    bp, nb = C.c_void_p(), C.c_uint64()
-    assert lib.b200_rec_finish(recs[0], C.byref(bp), C.byref(nb)) == 0
-    rblob = np.ctypeslib.as_array(C.cast(bp, C.POINTER(C.c_uint8)), shape=(nb.value,)).copy()
-    for r in recs:
-        lib.b200_rec_destroy(r)
-    return rblob
+        recs[0].merge(recs[k])
+    return recs[0].finish()
 
 
 def test_recorder_matches_numpy_builder(built):
     """the C recorder (host-only code path of libb200hevc.so) and the numpy builder produce equivalent blobs"""
-    from openhevc_b200 import _lib
-    lib = _lib.load()
     w, h, cfi, bd = 128, 64, 1, 8
     s = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=11, refs=[1, 2], cur_slot=3, exotic=0.05)
     blob, _ = s.generate()
     hdr, secs = W.parse_blob(blob)
-    rblob = replay_through_recorders(lib, blob, (w, h, cfi, bd), 1)
+    rblob = replay_through_recorders(blob, (w, h, cfi, bd), 1)
     # same picture on the oracle from both blobs
     dpb = [smooth_frame(w, h, cfi, bd, 50 + k) for k in range(4)]
     a = oracle_lib.execute(blob, dpb)
@@ -235,11 +236,9 @@ def test_recorder_matches_numpy_builder(built):
 def test_recorder_merge_of_worker_threads(built, n_workers, cfi, refs):
     """WPP / slice threads: per-worker recorders (CTB rows interleaved) merged at frame end give the same picture,
     and the merged intra list is still in a valid dependency order"""
-    from openhevc_b200 import _lib
-    lib = _lib.load()
     w, h, bd = 192, 320, 10
     blob, _ = FrameSynth(w, h, cfi=cfi, bit_depth=bd, seed=77 + n_workers, refs=refs, cur_slot=3, exotic=0.05, p_intra=0.3 if refs else 1.0).generate()
-    rblob = replay_through_recorders(lib, blob, (w, h, cfi, bd), n_workers)
+    rblob = replay_through_recorders(blob, (w, h, cfi, bd), n_workers)
     oracle_lib.check_decode_order(rblob)
     dpb = [smooth_frame(w, h, cfi, bd, 60 + k) for k in range(4)]
     a = oracle_lib.execute(blob, dpb)

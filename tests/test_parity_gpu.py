@@ -25,9 +25,7 @@ def run_sequence(w, h, cfi, bd, seeds, n_slots=4, check_order=True, **kw):
                 oracle_lib.check_decode_order(blob)
             got = eng.decode(blob)
             want = oracle_lib.execute(blob, dpb)
-            for p in range(3):
-                bad = np.argwhere(got[p] != want[p])
-                assert len(bad) == 0, f"picture {k} plane {p}: {len(bad)} samples differ, first at (y,x)={tuple(bad[0])} got {got[p][tuple(bad[0])]} want {want[p][tuple(bad[0])]}"
+            oracle_lib.assert_same(got, want, f"picture {k}")
             dpb[k] = [p.copy() for p in want]
     finally:
         eng.close()
@@ -72,8 +70,7 @@ def test_sao_restore_of_bypass_pus():
                 want = oracle_lib.execute(blob2, dpb)
                 plain = oracle_lib.execute(blob, dpb)
                 assert any((a != b).any() for a, b in zip(want, plain)), "the restore changed nothing"
-                for p in range(3):
-                    assert (got[p] == want[p]).all(), f"{w}x{h} cfi {cfi} bd {bd} seed {seed} plane {p}"
+                oracle_lib.assert_same(got, want, f"{w}x{h} cfi {cfi} bd {bd} seed {seed}")
         finally:
             eng.close()
 
@@ -115,13 +112,9 @@ def test_config_c3_4k_main10_b_picture():
             eng.upload_slot(s, dpb[s])
         blob, st = FrameSynth(w, h, cfi, bd, seed=81, refs=[1, 2], cur_slot=0).generate()
         got = eng.decode(blob)
-        want = oracle_lib.execute(blob, dpb)
-        for p in range(3):
-            assert (got[p] == want[p]).all()
+        oracle_lib.assert_same(got, oracle_lib.execute(blob, dpb), "4K picture")
         # size-independent properties: determinism of the whole pipeline and independence from arena / slot reuse
-        again = eng.decode(blob)
-        for p in range(3):
-            assert (again[p] == got[p]).all()
+        oracle_lib.assert_same(eng.decode(blob), got, "4K picture decoded again")
     finally:
         eng.close()
 
@@ -134,10 +127,7 @@ def test_config_c5_8k_422_main10():
         dpb = [smooth_frame(w, h, cfi, bd, 90 + k) for k in range(2)]
         eng.upload_slot(1, dpb[1])
         blob, st = FrameSynth(w, h, cfi, bd, seed=91, refs=[1], cur_slot=0, split_bias=0.4, coded_frac=0.3).generate()
-        got = eng.decode(blob)
-        want = oracle_lib.execute(blob, dpb)
-        for p in range(3):
-            assert (got[p] == want[p]).all()
+        oracle_lib.assert_same(eng.decode(blob), oracle_lib.execute(blob, dpb), "8K 4:2:2 picture")
     finally:
         eng.close()
 
@@ -152,15 +142,15 @@ def test_malformed_blobs_are_rejected_not_executed():
     eng = FrameEngine(128, 64, 1, 8, n_slots=2)
     try:
         blob, _ = FrameSynth(128, 64, 1, 8, seed=5, cur_slot=0).generate()
-        bad = blob.copy(); bad[0] ^= 0xFF
+        bad = blob.copy(); W.header(bad)["magic"] ^= 0xFF
         with pytest.raises(B200Error):
             eng.submit(bad)
-        bad = blob.copy(); bad[23] = 9                         # cur_slot out of range
+        bad = blob.copy(); W.header(bad)["cur_slot"] = 9       # out of range
         with pytest.raises(B200Error):
             eng.submit(bad)
         with pytest.raises(B200Error):
             eng.submit(blob[:1000])
-        bad = blob.copy(); bad[:256].view(W.header_dt)["reserved_section"]["count"] = 1     # reserved header field in use
+        bad = blob.copy(); W.header(bad)["reserved_section"]["count"] = 1     # reserved header field in use
         with pytest.raises(B200Error, match="reserved"):
             eng.submit(bad)
         eng.decode(blob)                                        # context still usable
@@ -218,9 +208,7 @@ def test_grey_reference_fill(cfi, bd):
             assert got[p].shape == eng.plane_shape(p) and (got[p] == grey).all()
             dpb[1][p][:] = grey
         blob, _ = FrameSynth(w, h, cfi, bd, seed=41, refs=[1], cur_slot=0, poc=1).generate()
-        pic, want = eng.decode(blob), oracle_lib.execute(blob, dpb)
-        for p in range(3):
-            assert np.array_equal(pic[p], want[p])
+        oracle_lib.assert_same(eng.decode(blob), oracle_lib.execute(blob, dpb), "picture predicted from the grey slot")
     finally:
         eng.close()
 
@@ -253,14 +241,8 @@ def ccp_blob(w, h, bd, seed, corrupt=False):
     """a 4:4:4 picture of cross-component-prediction blocks built through the recorder API the way the shim does it
     (hevcdsp_init_b200.c: rec_cross_component): luma block, the same luma block parked, the chroma block's own residual parked
     (or none), and the record that combines them -- half of the blocks intra predicted (result parked for the intra stage)"""
-    import ctypes as C
-    from openhevc_b200 import _lib
-    lib = _lib.load()
     rng = np.random.default_rng(seed)
-    cfg = _lib.B200Config(0, w, h, 3, bd, 6, 2, 2, 0, None, 0)
-    r = C.c_void_p()
-    assert lib.b200_rec_create(C.byref(cfg), C.byref(r)) == 0
-    assert lib.b200_rec_begin(r, 0, 0) == 0
+    rec = W.Recorder((w, h, 3, bd))
     for y in range(0, h, 16):
         for x in range(0, w, 16):
             log2 = int(rng.choice([2, 3, 4]))
@@ -274,28 +256,21 @@ def ccp_blob(w, h, bd, seed, corrupt=False):
                 return np.ascontiguousarray(c)
             cy = coeffs()
             if intra:
-                assert lib.b200_rec_intra(r, 0, x, y, log2, 1, 0, 0, 0) == 0
-            assert lib.b200_rec_tu(r, 0, x, y, log2, W.TU_IDCT, 0, n, cy.ctypes.data, -1) == 0
-            off_y = C.c_uint32()
-            assert lib.b200_rec_tu_parked(r, 0, x, y, log2, W.TU_IDCT, 0, n, cy.ctypes.data, C.byref(off_y)) == 0
+                rec.intra(0, x, y, log2, 1, 0, 0, 0)
+            rec.tu(0, x, y, log2, W.TU_IDCT, 0, n, cy, -1)
+            off_y = rec.tu_parked(0, x, y, log2, W.TU_IDCT, 0, n, cy)
             for plane in (1, 2):
                 if intra:
-                    assert lib.b200_rec_intra(r, plane, x, y, log2, 1, 0, 0, 0) == 0
+                    rec.intra(plane, x, y, log2, 1, 0, 0, 0)
                 has_c = bool(rng.integers(2))
-                off_c = C.c_uint32()
-                if has_c:
-                    cc = coeffs()
-                    assert lib.b200_rec_tu_parked(r, plane, x, y, log2, W.TU_IDCT, 0, n, cc.ctypes.data, C.byref(off_c)) == 0
+                off_c = rec.tu_parked(plane, x, y, log2, W.TU_IDCT, 0, n, coeffs()) if has_c else 0
                 scale = int(rng.choice([1, 2, 4, 8])) * int(rng.choice([-1, 1]))
-                assert lib.b200_rec_ccp(r, plane, x, y, log2, scale, off_y.value, int(has_c), off_c.value) == 0
-    blob_p, nbytes = C.c_void_p(), C.c_uint64()
-    assert lib.b200_rec_finish(r, C.byref(blob_p), C.byref(nbytes)) == 0
-    blob = np.ctypeslib.as_array(C.cast(blob_p, C.POINTER(C.c_uint8)), (nbytes.value,)).copy()
-    lib.b200_rec_destroy(r)
+                rec.ccp(plane, x, y, log2, scale, off_y, int(has_c), off_c)
+    blob = rec.finish()
     if corrupt:
-        hdr, _ = W.parse_blob(blob)
-        off = int(hdr["ccp"]["off"])
-        blob[off + 8:off + 12] = np.frombuffer(np.uint32(0x7fffff00).tobytes(), np.uint8)      # off_y of the first record far outside the pool
+        s = W.header(blob)["ccp"]
+        ccp = blob[int(s["off"]):int(s["off"]) + W.ccp_dt.itemsize * int(s["count"])].view(W.ccp_dt)
+        ccp["off_y"][0] = 0x7fffff00                           # the first record's luma residual far outside the pool
     return blob
 
 
@@ -312,15 +287,14 @@ def test_cross_component_prediction(bd):
             blob = ccp_blob(w, h, bd, seed)
             got = eng.decode(blob)
             want = oracle_lib.execute(blob, [[p.copy() for p in before], [np.zeros_like(p) for p in before]])
-            for p in range(3):
-                assert np.array_equal(got[p], want[p]), f"plane {p} differs (seed {seed})"
+            oracle_lib.assert_same(got, want, f"seed {seed}")
         with pytest.raises(B200Error, match="rejected on the device"):
             eng.decode(ccp_blob(w, h, bd, 3, corrupt=True))
         eng.upload_slot(0, before)
         blob = ccp_blob(w, h, bd, 1)
         again = eng.decode(blob)
         want = oracle_lib.execute(blob, [[p.copy() for p in before], [np.zeros_like(p) for p in before]])
-        assert all(np.array_equal(a, b) for a, b in zip(again, want))
+        oracle_lib.assert_same(again, want, "seed 1 after the rejected picture")
     finally:
         eng.close()
 
@@ -365,8 +339,7 @@ def test_out_of_order_lanes_keep_slot_hazards(lanes):
             recent = ([cur] + [s for s in recent if s != cur])[:4]
         eng.sync()
         for k, (got, want) in enumerate(zip(outs, wants)):
-            for p in range(3):
-                assert np.array_equal(got[p], want[p]), f"picture {k} plane {p} differs ({lanes} lanes)"
+            oracle_lib.assert_same(got, want, f"picture {k} ({lanes} lanes)")
     finally:
         eng.close()
 

@@ -11,13 +11,12 @@ boundary filters past both ends; and a layout that tiles the planes densely in z
 next TU through the edge records.  Blobs come from the C recorder (b200_rec_tu / b200_rec_intra / b200_rec_finish); the
 device must equal the CPU oracle, and where the reference's own tables are built (oracle/_ref/libreplay_ref.so) the
 oracle must equal them.  A numpy restatement counts how often each limit was really reached and fails if one never was."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import oracle_lib
-from openhevc_b200 import FrameEngine, B200Error, _lib
+from oracle_lib import assert_same
+from openhevc_b200 import FrameEngine, B200Error
 from openhevc_b200 import worklist as W
 
 pytestmark = pytest.mark.gpu
@@ -108,46 +107,6 @@ def residual(c, kind, flags, log2, col_limit, bd, count):
     return r
 
 
-# ---------------------------------------------------------------------------------------------------------------------
-# blobs through the C recorder
-# ---------------------------------------------------------------------------------------------------------------------
-class Recorder:
-    """one picture recorded the way the decoder's table calls arrive"""
-
-    def __init__(self, geom, cur_slot=0):
-        self.lib = _lib.load()
-        w, h, cfi, bd = geom
-        cfg = _lib.B200Config(0, w, h, cfi, bd, 6, 2, 2, 0, None, 0)
-        self.r = C.c_void_p()
-        assert self.lib.b200_rec_create(C.byref(cfg), C.byref(self.r)) == 0
-        assert self.lib.b200_rec_begin(self.r, cur_slot, 0) == 0
-
-    def tu(self, plane, x, y, log2, kind, flags, col_limit, coeffs, linked):
-        c = np.ascontiguousarray(coeffs, np.int16)
-        return self.lib.b200_rec_tu(self.r, plane, x, y, log2, kind, flags, col_limit, c.ctypes.data, linked)
-
-    def pcm(self, plane, x, y, log2, samples):
-        s = np.ascontiguousarray(samples, np.int16)
-        assert self.lib.b200_rec_pcm(self.r, plane, x, y, log2, s.ctypes.data) == 0
-
-    def intra(self, plane, x, y, log2, mode, flags, trs, bls):
-        assert self.lib.b200_rec_intra(self.r, plane, x, y, log2, mode, flags, trs, bls) == 0
-
-    def all_intra_cip(self, geom):
-        """constrained_intra_pred with every min-PU intra: the general intra path, availability unchanged"""
-        w, h = geom[0], geom[1]
-        ones = np.ones((h >> 2) * (w >> 2), np.uint8)
-        assert self.lib.b200_rec_set_cip(self.r, 2, w >> 2, h >> 2, ones.ctypes.data) == 0
-
-    def finish(self):
-        try:
-            bp, nb = C.c_void_p(), C.c_uint64()
-            assert self.lib.b200_rec_finish(self.r, C.byref(bp), C.byref(nb)) == 0
-            return np.ctypeslib.as_array(C.cast(bp, C.POINTER(C.c_uint8)), (nb.value,)).copy()
-        finally:
-            self.lib.b200_rec_destroy(self.r)
-
-
 def other_transport(blob, geom):
     """the same picture with every non-PCM TU in the other coefficient transport: dense blocks as (position, value) pairs of
     all their non-zero coefficients, pair lists as dense blocks (the recorder picks one form by density; both must agree)"""
@@ -173,12 +132,6 @@ def other_transport(blob, geom):
         tus[k + 2] = recs
     coeff = np.concatenate(parts) if parts else np.zeros(0, np.int16)
     return W.build_blob(w, h, cfi, bd, int(hdr["log2_ctb_size"]), int(hdr["cur_slot"]), coeff=coeff, tu=tus, intra=secs[W.SEC_INTRA].copy())
-
-
-def assert_same(got, want, what):
-    for p in range(3):
-        bad = np.argwhere(np.asarray(got[p]) != np.asarray(want[p]))
-        assert len(bad) == 0, f"{what} plane {p}: {len(bad)} samples differ, first at (y,x)={tuple(bad[0])} got {got[p][tuple(bad[0])]} want {want[p][tuple(bad[0])]}"
 
 
 def check_picture(eng, blob, cur, what):
@@ -274,7 +227,7 @@ def run_residual_sweep(geom, seed, impulse_step=1):
         pic = 0
         while any(queues.values()):
             cur = noise_planes(geom, rng)
-            rec = Recorder(geom)
+            rec = W.Recorder(geom)
             direct = []
             for plane in range(3):
                 pw, ph = W.plane_dims(w, h, cfi, plane)
@@ -296,12 +249,12 @@ def run_residual_sweep(geom, seed, impulse_step=1):
                             continue
                         if parked:
                             rec.intra(plane, x, y, log2, k % 35, 0, 0, 0)
-                            assert rec.tu(plane, x, y, log2, kind, flags, col_limit, wrap16(c), 1) == 0
+                            rec.tu(plane, x, y, log2, kind, flags, col_limit, wrap16(c), 1)
                             residual(c, kind, flags, log2, col_limit, bd, count)
                             count["parked"] += 1
                             continue
                         cur[plane][y:y + n, x:x + n] = (0, maxv, cur[plane][y:y + n, x:x + n])[k % 3]
-                        assert rec.tu(plane, x, y, log2, kind, flags, col_limit, wrap16(c), 0) == 0
+                        rec.tu(plane, x, y, log2, kind, flags, col_limit, wrap16(c), 0)
                         direct.append((plane, x, y, n, residual(c, kind, flags, log2, col_limit, bd, count)))
             blob = rec.finish()
             what = f"{geom} residual picture {pic}"
@@ -485,17 +438,17 @@ def run_intra_sweep(geom, seed, sizes=(2, 3, 4, 5)):
                 placed.append((plane, x, y, log2, mode, flags, trs, bls, resid))
                 intra_count(cur[plane], x, y, n, log2, plane, mode, flags, bd, count)
             for cip in ((False, True) if log2 <= 3 else (False,)):
-                rec = Recorder(geom)
+                rec = W.Recorder(geom)
                 for (plane, x, y, lg, mode, flags, trs, bls, resid) in placed:
                     rec.intra(plane, x, y, lg, mode, flags, trs, bls)
                     if resid is not None:
                         c = rng.integers(I16_MIN, I16_MAX + 1, (n, n)) if resid == "noise" else np.full((n, n), resid)
-                        assert rec.tu(plane, x, y, lg, W.TU_BYPASS, 0, n, c, 1) == 0
+                        rec.tu(plane, x, y, lg, W.TU_BYPASS, 0, n, c, 1)
                         if not cip:
                             count["resid_hi"] += int(resid == I16_MAX)
                             count["resid_lo"] += int(resid == I16_MIN)
                 if cip:
-                    rec.all_intra_cip(geom)
+                    rec.set_cip(2, np.ones((h >> 2, w >> 2)))           # every min-PU intra: the general path, availability unchanged
                     count["cip"] += 1
                 check_picture(eng, rec.finish(), cur, f"{geom} intra {n}x{n} picture {pic}{' cip' if cip else ''}")
     finally:
@@ -582,15 +535,15 @@ def run_dense_intra(geom, seed):
                     resid = (I16_MAX, I16_MIN, None, "noise")[(i + k) % 4] if rng.random() < 0.8 else None
                     plan.append((plane, x, y, log2, mode, f, trs, bls, resid))
             for cip in (False, True):
-                rec = Recorder(geom)
+                rec = W.Recorder(geom)
                 for (plane, x, y, log2, mode, f, trs, bls, resid) in plan:
                     rec.intra(plane, x, y, log2, mode, f, trs, bls)
                     if resid is not None:
                         n = 1 << log2
                         c = np.random.default_rng(x * 7 + y).integers(I16_MIN, I16_MAX + 1, (n, n)) if resid == "noise" else np.full((n, n), resid)
-                        assert rec.tu(plane, x, y, log2, W.TU_BYPASS if resid != "noise" else W.TU_IDCT, 0, n, c, 1) == 0
+                        rec.tu(plane, x, y, log2, W.TU_BYPASS if resid != "noise" else W.TU_IDCT, 0, n, c, 1)
                 if cip:
-                    rec.all_intra_cip(geom)
+                    rec.set_cip(2, np.ones((h >> 2, w >> 2)))
                 blob = rec.finish()
                 hdr, secs = W.parse_blob(blob)
                 intra = secs[W.SEC_INTRA]
@@ -615,9 +568,8 @@ def test_intra_dense_zorder(w, h, cfi, bd):
 def all_intra_cip(blob):
     """the same picture with every min-PU of its constrained_intra_pred bitmap intra"""
     out = blob.copy()
-    hdr = W.parse_blob(out)[0]
-    off, count = int(hdr["cip"]["off"]), int(hdr["cip"]["count"])
-    out[off + 16:off + 4 * count] = 0xff
+    cip = W.header(out)["cip"]
+    out[int(cip["off"]):][W.cip_header_dt.itemsize:4 * int(cip["count"])] = 0xff          # the bitmap behind the B200CipHeader
     return out
 
 
@@ -670,13 +622,13 @@ def test_rdpcm_on_transformed_or_pcm_blocks_is_rejected():
     rng = np.random.default_rng(3)
     coeffs8, coeffs4, pcm8 = rng.integers(-200, 200, (8, 8)), rng.integers(-200, 200, (4, 4)), rng.integers(0, 256, (8, 8))
     # the good picture: an IDCT 8x8, a DC 8x8, a DST 4x4 and a PCM 8x8 block, and skip / bypass blocks with rdpcm
-    rec = Recorder(geom)
-    assert rec.tu(0, 0, 0, 3, W.TU_IDCT, 0, 8, coeffs8, 0) == 0
-    assert rec.tu(0, 0, 8, 3, W.TU_DC, 0, 8, coeffs8, 0) == 0
-    assert rec.tu(0, 8, 0, 2, W.TU_DST, 0, 4, coeffs4, 0) == 0
+    rec = W.Recorder(geom)
+    rec.tu(0, 0, 0, 3, W.TU_IDCT, 0, 8, coeffs8, 0)
+    rec.tu(0, 0, 8, 3, W.TU_DC, 0, 8, coeffs8, 0)
+    rec.tu(0, 8, 0, 2, W.TU_DST, 0, 4, coeffs4, 0)
     rec.pcm(0, 16, 0, 3, pcm8)
-    assert rec.tu(0, 24, 0, 2, W.TU_SKIP, W.TUF_RDPCM | W.TUF_RDPCM_VERT, 4, coeffs4, 0) == 0
-    assert rec.tu(0, 32, 0, 3, W.TU_BYPASS, W.TUF_RDPCM, 8, coeffs8, 0) == 0
+    rec.tu(0, 24, 0, 2, W.TU_SKIP, W.TUF_RDPCM | W.TUF_RDPCM_VERT, 4, coeffs4, 0)
+    rec.tu(0, 32, 0, 3, W.TU_BYPASS, W.TUF_RDPCM, 8, coeffs8, 0)
     good = rec.finish()
     cur = noise_planes(geom, rng)
     eng = FrameEngine(*geom, n_slots=2, n_lanes=1)
@@ -695,8 +647,10 @@ def test_rdpcm_on_transformed_or_pcm_blocks_is_rejected():
             assert_same(eng.decode(good), first, f"good picture after rdpcm on kind {kind}")
     finally:
         eng.close()
-    rec = Recorder(geom)
+    rec = W.Recorder(geom)
     for kind, log2, c in ((W.TU_IDCT, 3, coeffs8), (W.TU_DST, 2, coeffs4), (W.TU_DC, 3, coeffs8), (W.TU_PCM, 3, pcm8)):
         for flags in (W.TUF_RDPCM, W.TUF_RDPCM | W.TUF_RDPCM_VERT):
-            assert rec.tu(0, 0, 0, log2, kind, flags, 1 << log2, c, 0) == -1, (kind, flags)      # B200_EINVAL
+            with pytest.raises(B200Error) as refused:
+                rec.tu(0, 0, 0, log2, kind, flags, 1 << log2, c, 0)
+            assert refused.value.code == -1, (kind, flags)      # B200_EINVAL
     rec.finish()

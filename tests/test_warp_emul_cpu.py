@@ -61,7 +61,7 @@ PARITY = ["test_weighted_prediction_and_sao_restore", "test_constrained_intra_pr
           "test_stages_individually", "test_far_out_of_picture_motion", "test_pcm_and_exotic_transform_paths", "test_malformed_blobs_are_rejected_not_executed",
           "test_malformed_inter_records_are_rejected_on_the_device", "test_empty_work_list_and_smallest_pictures"]
 # tests/test_mc_limits_gpu.py: inter prediction at the limits of its input space, and block-form lists that leave tiles unwritten
-MC_LIMITS = ["test_mc_block_with_tiles_in_two_buckets", "test_small_tile_region_need_not_be_bucket_ordered", "test_malformed_block_lists_are_rejected_on_the_device"]
+MC_LIMITS = ["test_mc_block_with_tiles_in_two_buckets", "test_small_tile_region_need_not_be_bucket_ordered", "test_block_lists_whose_tile_counts_or_places_disagree_are_rejected"]
 
 
 @needs_emul
@@ -203,7 +203,7 @@ def test_smoke_on_the_emulated_kernels(emulated, capsys):
     assert "smoke ok" in capsys.readouterr().out
 
 
-def test_address_sanitizer_sees_no_out_of_bounds_access_in_the_kernels():
+def test_address_sanitizer_sees_no_out_of_bounds_access_in_kernels_or_validation():
     """the emulated library built with -fsanitize=address: device allocations are exact-size heap blocks and shared memory is
     static storage, so a kernel reading or writing one element too far -- which a GPU run forgives silently -- aborts here.
     Includes the malformed work lists that the device-side validation must reject before any kernel trusts them."""
@@ -220,7 +220,7 @@ def test_address_sanitizer_sees_no_out_of_bounds_access_in_the_kernels():
             "T.test_malformed_blobs_are_rejected_not_executed()\n"
             "T.test_malformed_inter_records_are_rejected_on_the_device()\n"
             "import test_mc_limits_gpu as M\n"
-            "M.test_malformed_block_lists_are_rejected_on_the_device()\n"
+            "M.test_block_lists_whose_tile_counts_or_places_disagree_are_rejected()\n"
             "M.test_mc_sweep(1, 10)\n"
             "import test_residual_intra_limits_gpu as R\n"
             "R.test_rdpcm_on_transformed_or_pcm_blocks_is_rejected()\n"
